@@ -1,13 +1,17 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of the B200 quantised-decode engine on BASELINE.json's headline workload:
+"""bench.py -- decode tokens/s of the H100 (sm_90a) quantised-decode engine on BASELINE.json's headline workload:
 LLaMA2-7B OmniQuant W4A16 (per-channel), bs=1, ctx=2048, synthetic random-init weights and prompts.
 
     python bench.py --gpus N --steps K --warmup W           (N>1: launched by torch.distributed.run)
     python bench.py --impl reference ...                    (the reference path's CPU implementation)
+    python bench.py ... --dump-outputs DIR                  (also write the last timed step's outputs as DIR/<name>.npy)
 
 One "step" = one decode step (one token for the whole batch) through all 32 layers + lm_head.
   value      device-resident: tokens stay on the GPU (step -> argmax -> next step) in one CUDA graph;
              timed with CUDA events over exactly K steps, barrier + synchronize on both sides, max over ranks.
+             --dump-outputs DIR writes what the K-th step returned: logits.npy (fp32 [bsz, vocab]) and next_token.npy
+             (the argmax the loop feeds back, float64 [bsz]).  Weights, KV cache and first token are seeded, so the same
+             arguments give the same inputs on every run.
   e2e        the same K steps through the public drop-in API (Transformer.forward_inference): every step
              copies the token from pinned host memory, and reads the sampled token back to the host.
   roofline   the dequant-GEMV kernel (the only kernel that touches weights): algorithmic packed bytes of
@@ -59,21 +63,7 @@ def peaks():
     if os.path.isfile(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(kernel_name):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-    capture summary of this round (profiles/r02_ncu_traffic.json: {kernel substring: bytes}); None when not captured."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    try:
-        d = json.load(open(p))
-        for k, v in d.items():
-            if k in kernel_name:
-                return float(v)
-    except Exception:
-        pass
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -356,6 +346,8 @@ def main():
     ap.add_argument("--no-pdl", action="store_true")
     ap.add_argument("--bits", type=int, default=4)
     ap.add_argument("--group-size", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's logits and next token as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -455,6 +447,11 @@ def main():
             torch.cuda.synchronize()
             _log(f"step {i} ok")
     barrier()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), eng.greedy_logits[:BSZ].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "next_token.npy"), eng.tokens[:BSZ].cpu().numpy().astype(np.float64))
     total_ms = ev[0].elapsed_time(ev[K])
     per_step = sorted(ev[i].elapsed_time(ev[i + 1]) for i in range(K))
     clk = clocks.stop() if clocks else None
@@ -574,20 +571,18 @@ def main():
         "scaling": "strong", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": WORKLOAD, "bits": args.bits, "group_size": args.group_size, "bsz": BSZ, "ctx": CTX,
                    "parallelism": f"tp{world}", "p50_ms_per_token": p50, "p90_ms_per_token": per_step[int(K * 0.9)],
-                   "tokens_per_s_per_gpu": value / world, "l2": "inputs_exceed_l2 (3.5 GB of weights per step >> 126 MB)",
+                   "tokens_per_s_per_gpu": value / world, "l2": "inputs_exceed_l2 (3.5 GB of weights per step >> 50 MB)",
                    "pdl": eng.use_pdl, "cuda_graph": True, "step_bytes": sb,
-                   "step_hbm_frac_of_peak": step_frac, "step_hbm_frac_of_8TBps": sb["total"] / (p50 / 1000.0) / 8e12,
+                   "step_hbm_frac_of_peak": step_frac,
                    "prefill_2048_ms": prefill_ms,
-                   "prefill_path": "tcgen05 W4A16 GEMM (b200_prefill_gemm_w4) in 256-token chunks + decode-attention per 32 queries"},
+                   "prefill_path": "wgmma W4A16 GEMM (b200_prefill_gemm_w4) in 256-token chunks + decode-attention per 32 queries"},
         "clocks": clk,
         "e2e": {"value": e2e_value, "unit": "tokens/s", "h2d_bytes_per_step": 8 * BSZ, "d2h_bytes_per_step": 8 * BSZ},
         "gpu_launches": launches_per_step * K,
         "roofline": {"bound": "hbm", "kernel": kernel_name,
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "frac_of_8TBps": achieved / 8000.0,
                      "peak_source": peak_src, "bytes_per_launch_avg": bytes_per_launch,
-                     "launch_ms_avg": dom_ms / n_launch,
-                     "traffic": ncu_traffic(kernel_name)},
+                     "launch_ms_avg": dom_ms / n_launch},
     }
     if tp_parity is not None:
         out["tp_parity"] = tp_parity

@@ -1,5 +1,5 @@
 /*
- * b200_decode.h -- C ABI of libb200decode.so: the B200 (sm_100a) quantised-decode hot path that
+ * b200_decode.h -- C ABI of libb200decode.so: the H100 (sm_90a) quantised-decode hot path that
  * sits behind LLaMA2-Accessory's Transformer.forward_inference (accessory/model/LLM/llama.py:394-427,
  * mixtral.py:441-474) and its quantised-linear plug-in hook (accessory/util/quant.py:18-46,95-163).
  *
@@ -245,9 +245,9 @@ int b200_ipc_close(void* peer_ptr);
 int b200_ipc_free(void* own_ptr);
 
 /* ------------------------------------------------------------------------------------------------
- * Prefill (prompt) path on the 5th-generation tensor cores: out[T, N] = x[T, K] . w_hat[N, K]^T with
+ * Prefill (prompt) path on the Hopper tensor cores: out[T, N] = x[T, K] . w_hat[N, K]^T with
  * w_hat = fp16(fp16(q - z) * s16), the reference's fake-quantised weight reproduced bit for bit, fp32 accumulation in
- * tensor memory (tcgen05.mma, M = 128 weight rows per CTA, N = up to 256 tokens per launch, K = 64 per pipeline stage).
+ * registers (wgmma, M = 128 weight rows per CTA, N = up to 256 tokens per launch, K = 64 per pipeline stage).
  * Replaces F.linear at M = prompt tokens (quant.py:18-46) for per-channel W4 linears with N % 128 == 0, K % 64 == 0.
  * The elementwise kernels are the unfused forms of the decode GEMV's prologue / epilogues for T-token chunks:
  *   b200_prefill_rmsnorm   h = resid (+ delta) -> h_out (may be NULL); x = fp16(h * rsqrt(mean h^2 + eps)) * gamma

@@ -1,4 +1,4 @@
-"""llama2-accessory_b200: B200-native (sm_100a) quantised decode engine behind LLaMA2-Accessory's
+"""llama2-accessory_b200: H100-native (sm_90a) quantised decode engine behind LLaMA2-Accessory's
 MetaModel / Transformer.forward_inference / fairscale-style parallel-linear surface.
 
 Import as `llama2_accessory_b200` (the directory name carries a hyphen; the repo-root module

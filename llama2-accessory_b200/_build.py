@@ -1,4 +1,4 @@
-"""Build libb200decode.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200decode.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 Staleness is decided by a content hash of the sources (file times do not survive the copy to the GPU box), and the
 build is serialised with a file lock so that the ranks of a multi-process launch never compile concurrently."""
@@ -12,7 +12,7 @@ SRC = ["api.cu", "gemv.cu", "gemv1.cu", "mega1.cu", "mega2.cu", "attn.cu", "pref
 HDR = ["common.cuh", "gemv_core.cuh", "gemv1_core.cuh"]
 OUT = os.path.join(HERE, "libb200decode.so")
 STAMP = OUT + ".srchash"
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-shared"]
 
 

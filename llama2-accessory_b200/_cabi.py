@@ -146,7 +146,7 @@ def lib():
         if not os.path.isfile(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). The B200 decode engine has no CPU or PyTorch fallback.")
+                "(nvcc, sm_90a). The decode engine has no CPU or PyTorch fallback.")
         _lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(_lib, name)  # AttributeError if a declared symbol is not exported

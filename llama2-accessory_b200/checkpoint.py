@@ -493,7 +493,7 @@ def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, 
     meta = read_model_meta(pretrained_path, llama_type, llama_config)
     kind = _KIND_OF_TYPE.get(meta["llama_type"])
     if kind is None:
-        raise ValueError(f"llama_type {meta['llama_type']!r} is not served by the B200 decode engine")
+        raise ValueError(f"llama_type {meta['llama_type']!r} is not served by this decode engine")
     args = dict(meta["config"])
     args.setdefault("vocab_size", 32000)
     args["max_seq_len"], args["max_batch_size"] = max_seq_len, max_batch_size

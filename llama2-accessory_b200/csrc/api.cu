@@ -62,13 +62,13 @@ static void query() {
   if (g_sm) return;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) {
-    g_sm = 148;
+    g_sm = 132;
     g_smem = 227 * 1024;
     return;
   }
   int v = 0;
   cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-  g_sm = v > 0 ? v : 148;
+  g_sm = v > 0 ? v : 132;
   cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   g_smem = v > 0 ? (size_t)v : 227 * 1024;
 }

@@ -1,4 +1,4 @@
-// GQA decode attention with split-KV (flash-decoding) for sm_100a.
+// GQA decode attention with split-KV (flash-decoding) for sm_90a.
 //
 // Replaces repeat_kv + F.scaled_dot_product_attention / flash_attn_func for seqlen-1 queries
 // (accessory/model/LLM/llama.py:170-206).  The KV cache is stored as shared-memory images (see below), written
@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
   int s_begin, s_end, n_tiles;
   if (p.even) {
     // the 32-position tiles that hold keys are dealt out evenly (split i gets floor or ceil of n_t / n_split): with equal
-    // rounded-up chunks 2048 keys over 9 splits became 8 x 8 tiles + an idle split, i.e. 256 busy CTAs on 148 SMs (2 : 1)
+    // rounded-up chunks 2048 keys over 9 splits became 8 x 8 tiles + an idle split, i.e. 256 busy CTAs on 132 SMs (about 2 : 1)
     const int n_t = (kv_len + kTile - 1) / kTile;
     const int t_begin = (int)(((long long)n_t * split) / p.n_split), t_end = (int)(((long long)n_t * (split + 1)) / p.n_split);
     s_begin = t_begin * kTile;
@@ -445,9 +445,9 @@ extern "C" int b200_attn_choose_split(int T, int Hkv, int max_kv_len) {
   const int target = 2 * sm_count();
   int want = target / (T * Hkv);
   const int max_split = (max_kv_len + kChunkAlign - 1) / kChunkAlign;
-  // <= 8 splits merge through distributed shared memory (a portable cluster); more use the workspace merge.  Capping at 8
-  // measured SLOWER on B200 (676 vs 770 tokens/s, gpurun_out/r2d_bench.txt): a cluster is only scheduled once 8 CTA
-  // slots of one GPC are free at the same time, which defeats the early start under programmatic dependent launch.
+  // <= 8 splits merge through distributed shared memory (a portable cluster); more use the workspace merge.  The split
+  // count is not capped at 8: a cluster is only scheduled once 8 CTA slots of one GPC are free at the same time, which
+  // defeats the early start under programmatic dependent launch.
   const int cap = tune_get("B200_ATTN_MAX_SPLIT", 16);
   want = std::max(1, std::min(want, max_split));
   if (want > cap && T * Hkv * cap >= sm_count()) want = std::max(cap, 1);  // keep >= one CTA per SM when capping

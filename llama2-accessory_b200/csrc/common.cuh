@@ -1,4 +1,4 @@
-// Device-side helpers shared by the sm_100a kernels: mbarrier + 1-D bulk (TMA-engine) copies,
+// Device-side helpers shared by the sm_90a kernels: mbarrier + 1-D bulk (TMA-engine) copies,
 // warp-level HMMA, programmatic dependent launch, cache-hinted vector loads.
 #pragma once
 #include <cuda_fp16.h>
@@ -55,7 +55,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 
 // The same copy with an L2 cache-policy operand.  Weights and K/V tiles are read exactly once per decode step: with the
 // evict_first policy the 3.5 GB they add up to stop pushing everything else (kernel instructions, activation vectors,
-// norm weights, scales) out of the 126 MB L2 between two uses.
+// norm weights, scales) out of the 50 MB L2 between two uses.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -179,7 +179,7 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---- optional per-launch timeline (B200 %globaltimer, ns): [0]=first CTA start (min), [1]=x staged (max),
+// ---- optional per-launch timeline (%globaltimer, ns): [0]=first CTA start (min), [1]=x staged (max),
 // [2]=last MMA warp done (max), [3]=last CTA end (max).  tl == nullptr -> off.
 __device__ __forceinline__ unsigned long long gtime_ns() {
   unsigned long long t;

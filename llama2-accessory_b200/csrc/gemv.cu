@@ -1,4 +1,4 @@
-// Fused W{2,3,4,16}A16 dequant-GEMV family for decode (T <= 32 tokens), sm_100a.
+// Fused W{2,3,4,16}A16 dequant-GEMV family for decode (T <= 32 tokens), sm_90a.
 //
 //   prologue : optional residual add + RMSNorm (components.py:41-53), x staged once per CTA in smem
 //   main loop: packed weights streamed HBM -> smem ring by 1-D TMA bulk copies (UBLKCP) issued by a
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemv_kernel(const __grid_constant
       }
       // Own stream fully issued: pull this CTA's share of the NEXT kernel's first bytes into L2, so HBM keeps
       // streaming through our epilogue, the launch gap and the next kernel's prologue (one CTA per SM leaves
-      // no room for a co-resident successor; the 126 MB L2 is the hand-over buffer instead).
+      // no room for a co-resident successor; the 50 MB L2 is the hand-over buffer instead).
       if (p.next_w && p.next_bytes > 0)
         prefetch_next_stream(p.next_w, p.next_bytes, p.next_tiles, p.next_grid, p.next_window, blockIdx.x, gridDim.x);
     }
@@ -407,7 +407,7 @@ extern "C" int b200_gemv(const b200_gemv_args_t* a, b200_stream_t stream) {
   want = std::max(2, std::min(want, 24));
   // The activations of all tokens of a launch are staged in shared memory beside the weight ring.  When T*K is too
   // large for that (e.g. T = 32 at K = 4096, T = 8 at K = 11008) the batch is walked in token groups: one launch per
-  // group over the same weights, which the second and later groups find in the 126 MB L2.
+  // group over the same weights, which the second and later groups find in the 50 MB L2.
   int stages = 0;
   const int tg = pick_token_group(a->T, p0.n_chunk64, p0.x_stride, cap, want, &stages);
   if (tg <= 0) {

@@ -1,4 +1,4 @@
-// bs = 1 decode GEMV on the INTEGER tensor path (sm_100a): y = s * (sum_k q[n,k] x[k] - z * sum_k x[k]), exact.
+// bs = 1 decode GEMV on the INTEGER tensor path (sm_90a): y = s * (sum_k q[n,k] x[k] - z * sum_k x[k]), exact.
 //
 // Why a second kernel: at one token per step the fp16 HMMA kernel (gemv.cu) is bound by the ALU work of turning
 // packed nibbles into fp16 A fragments (20 SHF/LOP3 per 1024 weights and lane) and by ~4 us of fixed latency per

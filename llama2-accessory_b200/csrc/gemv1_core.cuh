@@ -66,7 +66,7 @@ constexpr int kProAttnMerge = 2;
 // Template value "decided at run time from p.pro / p.epi".  The stand-alone kernel (gemv1.cu) is ONE instance for all four
 // launches of a layer: with one instance per (prologue, epilogue) pair every launch started on instructions that the 3.5 GB
 // of weights streamed since their last use had pushed out of the L2 -- the activation staging alone took ~2.6 us of
-// instruction-fetch stalls (profiles/r02s_*).  A shared instance is re-executed every ~10 us and stays cached.
+// instruction-fetch stalls.  A shared instance is re-executed every ~10 us and stays cached.
 constexpr int kDyn = -1;
 
 // ring position (MMA warps and producer each keep their own copy) + tile counter of the partial-sum hand-off

@@ -4,8 +4,8 @@
 //   -> residual + RMSNorm + lm_head -> fp32 logits                                      (llama.py:394-427, 276-288)
 //
 // Why: as separate kernels every one of the 5L+1 dependent phases costs a drain, a dependency release, an x-staging
-// round trip and a cold ring (~3-4 us each, profiles/r02_timeline_*.txt) during which HBM idles; together that was more
-// than the 0.7 ms the step's 4.6 GB take at full bandwidth.  Here one CTA per SM stays resident for the whole step:
+// round trip and a cold ring during which HBM idles; together that is comparable to the time the step's
+// 4.6 GB take at full bandwidth.  Here one CTA per SM stays resident for the whole step:
 //   * the producer warp streams weights / K-V tiles of phase after phase through ONE shared-memory ring and never
 //     waits for a dependency (weights are constants); while the MMA warps sit at a grid barrier and re-stage the
 //     activation vector, the ring (~150 KB per SM = 3.4 us of HBM time) keeps filling, so HBM does not idle;

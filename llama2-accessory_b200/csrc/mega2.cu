@@ -1,9 +1,9 @@
 // Persistent whole-step kernel, DATAFLOW version: one bs = 1 decode step of a dense LLaMA per launch and tensor-parallel
 // rank, WITHOUT grid barriers.  (mega1.cu is the grid-barrier version of the same step.)
 //
-// What the timeline of mega1 showed (profiles/r02d_timeline_persistent_kernel.txt): every phase boundary cost
-// three dependent global round trips under streaming load -- stores + fence + arrive, poll the counter, load x -- about
-// 6 us per phase, five phases per layer.  Here every vector that crosses CTAs travels in the "flag-in-data" format of
+// What the timeline of mega1 showed: every phase boundary cost
+// three dependent global round trips under streaming load -- stores + fence + arrive, poll the counter, load x -- five
+// phases per layer.  Here every vector that crosses CTAs travels in the "flag-in-data" format of
 // low-latency collectives (NCCL's LL protocol): 8-byte units {payload, sequence number}, written with one 8-byte store
 // (single-copy atomic) and polled by the consumer until the sequence number of the producing phase appears.  A consumer
 // therefore sees its input ONE round trip after the producer's store lands; there is no fence, no counter, no barrier:
@@ -79,8 +79,7 @@ struct Params {
 
 // "The producers of phase ph are probably done" hint: one relaxed counter per phase, bumped (no fence) by every CTA after
 // its LL stores and watched by ONE thread per consumer CTA.  It only gates WHEN the consumers start polling the data (75 000
-// threads spinning on not-yet-written units took about half of the L2's request rate, profiles/r02g_timeline_dataflow_kernel
-// .txt); correctness still rests on the sequence numbers inside the data.
+// threads spinning on not-yet-written units took about half of the L2's request rate); correctness still rests on the sequence numbers inside the data.
 __device__ __forceinline__ unsigned* hint_ptr(const Params& mp, int rank, int ph) {
   return reinterpret_cast<unsigned*>(mp.comm[rank] + mp.lay.ctl + 64) + ph;
 }

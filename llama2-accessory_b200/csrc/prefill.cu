@@ -1,26 +1,29 @@
-// W4A16 prefill GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulator in tensor memory) and the elementwise
-// kernels around it; replaces F.linear at M = prompt tokens (accessory/util/quant.py:18-46, llama.py:276-288) for prompts
-// longer than one 32-token chunk of the decode GEMV.  First run on B200: gpurun_out/r2e_prefill.txt (5 shapes, max error
-// 1e-3 at |out| ~ 3 = fp16 rounding of the output).
+// W4A16 prefill GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers) and the elementwise kernels
+// around it; replaces F.linear at M = prompt tokens (accessory/util/quant.py:18-46, llama.py:276-288) for prompts longer
+// than one 32-token chunk of the decode GEMV.
 //
 // GEMM:   out[T, N] = x[T, K] . w_hat[N, K]^T
 //   w_hat = fp16(fp16(q - z) * s16)  -- the reference's fake-quantised weight, reproduced bit for bit, so the prefill
 //   logits follow F.linear(x, w_hat) with fp32 accumulation (accessory/util/quant.py:18-46 + SURVEY.md 8c).
 //
 // One CTA owns 128 output rows (eight 16-row tiles of the packed decode format, DESIGN.md section 3) and up to 256
-// tokens; D = A . B^T with A = dequantised weights [128 x 64] fp16, B = activations [T x 64] fp16, both K-major with
-// the 128-byte swizzle in shared memory, D [128 lanes x T columns] fp32 in tensor memory.
+// tokens.  D[rows x tokens] = A . B^T with A = dequantised weights (wgmma register operand), B = activations [T_pad x 64]
+// fp16 per k-block in shared memory (K-major, 128-byte swizzle), D in registers (fp32).
 //
-// Warp roles (12 warps):
-//   0..3   epilogue: tcgen05.ld of TMEM lanes 32*(warp%4).., fp32 -> fp16, out[t][row] stores
-//   4      producer: packed W4 k-blocks HBM -> smem (8 bulk copies of 512 B per k-block, mbarrier expect_tx)
-//   5      MMA issuer: one elected lane issues 4 x tcgen05.mma (M128, N = T_pad, K16) per k-block, tcgen05.commit
-//   6..7   activation loaders: x[T][kb*64 .. +64] -> swizzled B stage (cp.async 16 B, L2-resident source)
-//   8..11  dequant: packed stage -> fp16 A stage in the UMMA canonical layout (each uint4 of the decode format holds
-//          four 16-byte chunks: rows g / g+8 x two consecutive 8-k runs), fence.proxy.async, arrive
+// Warp roles (12 warps, three warpgroups; setmaxnreg moves registers from the third to the accumulators of the first two):
+//   0..7   two consumer warpgroups; warp w owns the 16-row tile w.  Per k-block: ld.shared of its packed uint4, dequant
+//          into four m64k16 A fragments, 4 x NC wgmma m64n32k16 (NC = T_pad / 32), wait; fp16 stores at the end
+//   8      producer: packed W4 k-blocks HBM -> smem (8 bulk copies of 512 B per k-block, mbarrier expect_tx)
+//   9..10  activation loaders: x[T][kb*64 .. +64] -> B stage, k permuted to the order of the packed fragments (below)
+//   11     idle
 //
-// Pipelines: packed_full/empty (producer <-> dequant), a_full + b_full -> MMA, ab_empty (tcgen05.commit -> loaders and
-// dequant), tmem_full (last commit -> epilogue).
+// k order inside a 64-wide k-block.  Lane (g, t) of a packed tile holds rows g, g+8 at physical k 16t .. 16t+15 (four
+// words: row g / g+8 x k 16t+0..7 / 16t+8..15), so the A fragment of k-step j is built from its own registers when
+// logical k 16j + 8h + 2t + e (the fragment position, e = 0, 1) stands for physical k 16t + 8h + 2j + e.  The loaders
+// store the activations in that logical order; the k-sum is the same sum.
+//
+// Pipelines: pk_full (bulk copies -> consumers), b_full (loaders -> consumers), empty (consumers, after the wgmma that read
+// the stage completed -> producer and loaders).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,21 +38,20 @@
 namespace b200 {
 namespace prefill {
 
-constexpr int BM = 128, BK = 64, kStages = 4, kMaxT = 256;
-constexpr int kThreads = 12 * 32;
-constexpr int kABytes = BM * BK * 2;        // 16 KB
+constexpr int BM = 128, BK = 64, kStages = 4, kMaxT = 256, kNChunk = 32;
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = (kConsumerWarps + 4) * 32;
 constexpr int kBBytes = kMaxT * BK * 2;     // 32 KB
 constexpr int kPackedBytes = 8 * 512;       // 4 KB: one k-block of eight 16-row tiles
+constexpr size_t kSmemBytes = (size_t)kStages * (kBBytes + kPackedBytes) + 3 * kStages * 8 + 1024;
 
 struct Params {
   const uint8_t* qw;     // packed W4, tile-major (b200_pack_weight)
   const __half2* sz;     // per-channel (s, z) [N]
   const __half* x;       // [T][K]
   __half* out;           // [T][N]
-  int N, K, KB, T, T_pad;  // T_pad = T rounded up to 16 (UMMA N), <= 256
+  int N, K, KB, T, T_pad;  // T_pad = NC * 32 >= T, <= 256
 };
-
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // K-major, SWIZZLE_128B canonical layout of a [rows x 64] fp16 tile: 8-row groups of 1024 B, 16-byte chunk c of row r
 // stored at chunk (c ^ (r & 7)).
@@ -57,37 +59,34 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
 }
 
-// cute::UMMA::SmemDescriptor (mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// layout type [61,64) (2 = SWIZZLE_128B).  K-major, one swizzle atom wide: SBO = 1024 B between 8-row groups.
+// wgmma shared-memory matrix descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), base offset [49,52),
+// layout type [62,64) (1 = SWIZZLE_128B).  K-major, one swizzle atom wide: LBO unused (1), SBO = 1024 B between 8-row
+// groups; the stage base is 1024-byte aligned, so the base offset is 0.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3ffff) >> 4);
-  d |= (uint64_t)0 << 16;                 // leading byte offset: unused for a single 128-byte atom along K
-  d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset
-  d |= (uint64_t)1 << 46;                 // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
-// cute::UMMA::InstrDescriptor for kind::f16: D = F32 (c_format 1 at [4,6)), A = B = F16 (0), both K-major,
-// n_dim = N >> 3 at [17,23), m_dim = M >> 4 at [24,29).
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
+// D[64 x 32] += A[64 x 16] (registers, fp16) . B[32 x 16]^T (shared memory, fp16, K-major), fp32 accumulate
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar))
-               : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // (q - z) * s as the reference rounds it: q as 1024 + q (exact in fp16), minus (1024 + z) (exact), times s (one rounding)
@@ -96,162 +95,133 @@ __device__ __forceinline__ uint32_t deq2(uint32_t nib2, __half2 zoff, __half2 s2
   const __half2 h = __hmul2(__hsub2(*reinterpret_cast<const __half2*>(&v), zoff), s2);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-// one packed u32 (8 consecutive k of one row, nibble order of pack.cpp kW4Nib) -> one 16-byte fp16 chunk
-__device__ __forceinline__ uint4 dequant_word(uint32_t w, __half2 sz) {
-  const __half s = __low2half(sz), z = __high2half(sz);
-  const __half2 s2 = __half2half2(s);
-  const __half2 zoff = __hadd2(__half2half2(z), __float2half2_rn(1024.f));  // 1024 + z: exact for |z| <= 1024
-  uint4 o;
-  o.x = deq2(w & 0x000f000fu, zoff, s2);          // k 0, 1
-  o.y = deq2((w >> 8) & 0x000f000fu, zoff, s2);   // k 2, 3
-  o.z = deq2((w >> 4) & 0x000f000fu, zoff, s2);   // k 4, 5
-  o.w = deq2((w >> 12) & 0x000f000fu, zoff, s2);  // k 6, 7
-  return o;
+// k pair 2j, 2j+1 of one packed u32 (8 consecutive k of one row, nibble order of pack.cpp kW4Nib: pairs at shifts
+// 0, 8, 4, 12)
+template <int J>
+__device__ __forceinline__ uint32_t deq_pair(uint32_t w, __half2 zoff, __half2 s2) {
+  constexpr int kShift = (J & 1) * 8 + (J >> 1) * 4;
+  return deq2((w >> kShift) & 0x000f000fu, zoff, s2);
 }
 
+template <int NC>
 __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __grid_constant__ Params p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* a_st = smem;                                   // [kStages][16 KB]
-  uint8_t* b_st = a_st + kStages * kABytes;               // [kStages][32 KB]
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);  // swizzle atoms need 1024-byte alignment
+  uint8_t* b_st = smem;                                   // [kStages][32 KB]
   uint8_t* pk_st = b_st + kStages * kBBytes;              // [kStages][4 KB]
   uint64_t* bars = reinterpret_cast<uint64_t*>(pk_st + kStages * kPackedBytes);
-  uint64_t* pk_full = bars;                 // [kStages] producer -> dequant (tx bytes)
-  uint64_t* pk_empty = pk_full + kStages;   // [kStages] dequant (128) -> producer
-  uint64_t* a_full = pk_empty + kStages;    // [kStages] dequant (128) -> MMA
-  uint64_t* b_full = a_full + kStages;      // [kStages] loaders (64) -> MMA
-  uint64_t* ab_empty = b_full + kStages;    // [kStages] tcgen05.commit -> dequant + loaders
-  uint64_t* tmem_full = ab_empty + kStages; // [1]
-  __shared__ uint32_t s_tmem;
+  uint64_t* pk_full = bars;                 // [kStages] producer -> consumers (tx bytes)
+  uint64_t* b_full = pk_full + kStages;     // [kStages] loaders (64) -> consumers
+  uint64_t* empty = b_full + kStages;       // [kStages] consumer warps (8) -> producer + loaders
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int row0 = blockIdx.x * BM;  // first output row of this CTA
   const int tile0 = row0 >> 4;
-  constexpr uint32_t kTmemCols = 256;
 
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&pk_full[s], 1);
-      mbar_init(&pk_empty[s], 128);
-      mbar_init(&a_full[s], 128);
       mbar_init(&b_full[s], 64);
-      mbar_init(&ab_empty[s], 1);
+      mbar_init(&empty[s], kConsumerWarps);
     }
-    mbar_init(tmem_full, 1);
     fence_mbar_init();
   }
-  if (warp == 0) {  // TMEM allocation by one warp (the same warp frees it)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(&s_tmem)), "n"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  fence_before();
   __syncthreads();
-  fence_after();
-  const uint32_t tmem = s_tmem;
 
-  if (warp == 4) {
+  if (warp < kConsumerWarps) {
+    // ---------------- consumers: dequant -> wgmma, then the fp16 epilogue ----------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    const int g = lane >> 2, t4 = lane & 3;
+    const __half2 sz_lo = p.sz[row0 + warp * 16 + g], sz_hi = p.sz[row0 + warp * 16 + g + 8];
+    const __half2 s_lo = __half2half2(__low2half(sz_lo)), s_hi = __half2half2(__low2half(sz_hi));
+    // 1024 + z: exact for |z| <= 1024
+    const __half2 z_lo = __hadd2(__half2half2(__high2half(sz_lo)), __float2half2_rn(1024.f));
+    const __half2 z_hi = __hadd2(__half2half2(__high2half(sz_hi)), __float2half2_rn(1024.f));
+    float acc[NC][16];
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
+    for (int kb = 0; kb < p.KB; ++kb) {
+      const int s = kb % kStages;
+      const uint32_t par = (kb / kStages) & 1;
+      mbar_wait(&pk_full[s], par);
+      const uint4 w = lds_v4(pk_st + s * kPackedBytes + warp * 512 + lane * 16);
+      // words: [0] row g, k 16t4 + 0..7; [1] row g+8, same k; [2] row g, k 16t4 + 8..15; [3] row g+8, same k
+      uint32_t a[4][4];
+#define B200_FRAG(J)                               \
+  a[J][0] = deq_pair<J>(w.x, z_lo, s_lo);          \
+  a[J][1] = deq_pair<J>(w.y, z_hi, s_hi);          \
+  a[J][2] = deq_pair<J>(w.z, z_lo, s_lo);          \
+  a[J][3] = deq_pair<J>(w.w, z_hi, s_hi);
+      B200_FRAG(0) B200_FRAG(1) B200_FRAG(2) B200_FRAG(3)
+#undef B200_FRAG
+      mbar_wait(&b_full[s], par);
+      const uint32_t b0 = smem_u32(b_st + s * kBBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < BK / 16; ++j)  // +32 bytes per K = 16 step inside the 128-byte swizzle atom
+#pragma unroll
+        for (int c = 0; c < NC; ++c)     // +32 rows (4 swizzle atoms of 8 rows) per n-chunk
+          wgmma_m64n32k16(acc[c], a[j], make_desc(b0 + c * 4096 + j * 32));
+      wgmma_commit();
+      wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);  // this warp's reads of the packed and B stages are complete
+    }
+    // D fragment of warp w: acc[c][4i + 2h + e] = (row 16w + g + 8h, token 32c + 8i + 2t4 + e)
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int t = c * 32 + i * 8 + 2 * t4 + e, row = row0 + warp * 16 + g + 8 * h;
+            if (t < p.T && row < p.N) p.out[(size_t)t * p.N + row] = __float2half_rn(acc[c][4 * i + 2 * h + e]);
+          }
+  } else {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+  }
+  if (warp == kConsumerWarps) {
     // ---------------- producer: packed weights ----------------
     if (lane == 0) {
       for (int kb = 0; kb < p.KB; ++kb) {
         const int s = kb % kStages;
         const uint32_t par = (kb / kStages) & 1;
-        mbar_wait(&pk_empty[s], par ^ 1);
+        mbar_wait(&empty[s], par ^ 1);
         mbar_arrive_expect_tx(&pk_full[s], kPackedBytes);
         for (int i = 0; i < 8; ++i)
           bulk_g2s(pk_st + s * kPackedBytes + i * 512, p.qw + ((size_t)(tile0 + i) * p.KB + kb) * 512, 512, &pk_full[s]);
       }
     }
-  } else if (warp == 5) {
-    // ---------------- MMA issuer ----------------
-    const uint32_t idesc = make_idesc(p.T_pad);
+  } else if (warp == kConsumerWarps + 1 || warp == kConsumerWarps + 2) {
+    // ---------------- activation loaders: x block -> B stage in fragment k order ----------------
+    // logical chunk c = 2j + h, word t  <-  physical word 4h + j + 8t  =  component j of input uint4 h + 2t
+    const int lt = tid - (kConsumerWarps + 1) * 32;  // 0..63
     for (int kb = 0; kb < p.KB; ++kb) {
       const int s = kb % kStages;
       const uint32_t par = (kb / kStages) & 1;
-      mbar_wait(&a_full[s], par);
-      mbar_wait(&b_full[s], par);
-      fence_after();
-      if (lane == 0) {
-        const uint32_t a0 = smem_addr(a_st + s * kABytes), b0 = smem_addr(b_st + s * kBBytes);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // +32 bytes per K = 16 step inside the 128-byte swizzle atom
-          umma_f16(tmem, make_desc(a0 + k * 32), make_desc(b0 + k * 32), idesc, (kb | k) ? 1u : 0u);
-        umma_commit(&ab_empty[s]);                 // frees the A / B stage when these MMAs have read it
-        if (kb == p.KB - 1) umma_commit(tmem_full);  // accumulator complete
-      }
-      __syncwarp();
-    }
-  } else if (warp == 6 || warp == 7) {
-    // ---------------- activation loaders: x block -> swizzled B stage ----------------
-    const int lt = tid - 6 * 32;  // 0..63
-    for (int kb = 0; kb < p.KB; ++kb) {
-      const int s = kb % kStages;
-      const uint32_t par = (kb / kStages) & 1;
-      mbar_wait(&ab_empty[s], par ^ 1);
+      mbar_wait(&empty[s], par ^ 1);
       uint8_t* dst = b_st + s * kBBytes;
-      for (int i = lt; i < p.T_pad * 8; i += 64) {
-        const int t = i >> 3, c = i & 7;
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (t < p.T) v = *reinterpret_cast<const uint4*>(p.x + (size_t)t * p.K + (size_t)kb * BK + c * 8);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(t, c)) = v;
+      for (int i = lt; i < p.T_pad * 2; i += 64) {
+        const int t = i >> 1, h = i & 1;
+        uint4 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          v[u] = make_uint4(0, 0, 0, 0);
+          if (t < p.T) v[u] = *reinterpret_cast<const uint4*>(p.x + (size_t)t * p.K + (size_t)kb * BK + (h + 2 * u) * 8);
+        }
+        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 0 + h)) = make_uint4(v[0].x, v[1].x, v[2].x, v[3].x);
+        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 + h)) = make_uint4(v[0].y, v[1].y, v[2].y, v[3].y);
+        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 4 + h)) = make_uint4(v[0].z, v[1].z, v[2].z, v[3].z);
+        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 6 + h)) = make_uint4(v[0].w, v[1].w, v[2].w, v[3].w);
       }
       fence_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
       mbar_arrive(&b_full[s]);
     }
-  } else if (warp >= 8) {
-    // ---------------- dequant: packed stage -> fp16 A stage ----------------
-    const int dt = tid - 8 * 32;  // 0..127: two (tile, lane) slots of the 8 x 32 per k-block
-    __half2 szr[2][2];
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      const int slot = dt + u * 128, ti = slot >> 5, g = (slot & 31) >> 2;
-      szr[u][0] = p.sz[row0 + ti * 16 + g];
-      szr[u][1] = p.sz[row0 + ti * 16 + g + 8];
-    }
-    for (int kb = 0; kb < p.KB; ++kb) {
-      const int s = kb % kStages;
-      const uint32_t par = (kb / kStages) & 1;
-      mbar_wait(&pk_full[s], par);
-      mbar_wait(&ab_empty[s], par ^ 1);
-      uint8_t* dst = a_st + s * kABytes;
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int slot = dt + u * 128, ti = slot >> 5, ln = slot & 31, g = ln >> 2, t4 = ln & 3;
-        const uint4 w = *reinterpret_cast<const uint4*>(pk_st + s * kPackedBytes + ti * 512 + ln * 16);
-        const int r_lo = ti * 16 + g, r_hi = r_lo + 8;
-        // words: [0] row g, k-run first half; [1] row g+8, first half; [2] row g, second half; [3] row g+8, second half
-        *reinterpret_cast<uint4*>(dst + sw128_offset(r_lo, t4 * 2 + 0)) = dequant_word(w.x, szr[u][0]);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(r_hi, t4 * 2 + 0)) = dequant_word(w.y, szr[u][1]);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(r_lo, t4 * 2 + 1)) = dequant_word(w.z, szr[u][0]);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(r_hi, t4 * 2 + 1)) = dequant_word(w.w, szr[u][1]);
-      }
-      fence_async_smem();
-      mbar_arrive(&a_full[s]);
-      mbar_arrive(&pk_empty[s]);
-    }
-  } else {
-    // ---------------- epilogue (warps 0..3): TMEM lanes 32*warp.. = output rows ----------------
-    mbar_wait(tmem_full, 0);
-    fence_after();
-    const int row = row0 + warp * 32 + lane;
-    for (int c0 = 0; c0 < p.T_pad; c0 += 16) {
-      uint32_t r[16];
-      const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-            "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int t = c0 + j;
-        if (t < p.T && row < p.N) p.out[(size_t)t * p.N + row] = __float2half_rn(__uint_as_float(r[j]));
-      }
-    }
   }
-
-  fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(kTmemCols));
 }
 
 }  // namespace prefill
@@ -346,28 +316,34 @@ extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, voi
     set_error("prefill_gemm_w4: per-channel W4 linear with N % 128 == 0 and K % 64 == 0 required");
     return B200_E_UNSUPPORTED;
   }
-  const size_t smem = (size_t)kStages * (kABytes + kBBytes + kPackedBytes) + 64 * 8 + 1024;
+  static void (*const kernels[kMaxT / kNChunk])(Params) = {
+      prefill_gemm_w4_kernel<1>, prefill_gemm_w4_kernel<2>, prefill_gemm_w4_kernel<3>, prefill_gemm_w4_kernel<4>,
+      prefill_gemm_w4_kernel<5>, prefill_gemm_w4_kernel<6>, prefill_gemm_w4_kernel<7>, prefill_gemm_w4_kernel<8>};
   static bool configured[16] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   dev &= 15;
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(prefill_gemm_w4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      set_error(std::string("prefill_gemm_w4: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-      return (int)e;
+    for (auto k : kernels) {
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+      if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        set_error(std::string("prefill_gemm_w4: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
+        return (int)e;
+      }
     }
     configured[dev] = true;
   }
-  for (int t0 = 0; t0 < T; t0 += kMaxT) {  // token blocks of <= 256: the accumulator of a CTA is 128 lanes x 256 columns of TMEM
+  for (int t0 = 0; t0 < T; t0 += kMaxT) {  // token blocks of <= 256: a CTA's accumulators are 128 rows x 256 fp32 registers
     Params p;
     p.qw = static_cast<const uint8_t*>(lin->qweight);
     p.sz = static_cast<const __half2*>(lin->scales);
     p.x = static_cast<const __half*>(x) + (size_t)t0 * lin->K;
     p.out = static_cast<__half*>(out) + (size_t)t0 * lin->N;
-    p.N = lin->N, p.K = lin->K, p.KB = lin->K / BK, p.T = std::min(kMaxT, T - t0), p.T_pad = (p.T + 15) / 16 * 16;
-    prefill_gemm_w4_kernel<<<lin->N / BM, kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
+    p.N = lin->N, p.K = lin->K, p.KB = lin->K / BK, p.T = std::min(kMaxT, T - t0);
+    const int nc = (p.T + kNChunk - 1) / kNChunk;
+    p.T_pad = nc * kNChunk;
+    kernels[nc - 1]<<<lin->N / BM, kThreads, kSmemBytes, static_cast<cudaStream_t>(stream)>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

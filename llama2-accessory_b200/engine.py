@@ -1,4 +1,4 @@
-"""DecodeEngine: the per-rank driver of the B200 decode hot path.
+"""DecodeEngine: the per-rank driver of the H100 (sm_90a) decode hot path.
 
 It owns the packed weights, the KV cache (engine layouts, see kvlayout.py / b200_decode.h: K [B][Hkv][S][128]
 chunk-swizzled, V [B][Hkv][S/32][128][32]) and the small activation buffers, and enqueues one decode step as
@@ -153,7 +153,7 @@ def check_kernel_limits(cfg: "EngineConfig"):
 class DecodeEngine:
     def __init__(self, cfg: EngineConfig, device="cuda", group=None):
         if cfg.head_dim != 128:
-            raise ValueError("the B200 decode kernels are specialised for head_dim = 128")
+            raise ValueError("the decode kernels are specialised for head_dim = 128")
         if cfg.n_heads % cfg.tp_world or cfg.kv_heads % cfg.tp_world:
             raise ValueError("n_heads and n_kv_heads must be divisible by the tensor-parallel size")
         check_kernel_limits(cfg)
@@ -195,7 +195,7 @@ class DecodeEngine:
         self.mega_dataflow = _m == 2
         self._mega = None
         self.mega_timeline = None
-        # prompts longer than one 32-token chunk: tcgen05 W4A16 GEMM (csrc/prefill.cu) instead of re-streaming the weights
+        # prompts longer than one 32-token chunk: wgmma W4A16 GEMM (csrc/prefill.cu) instead of re-streaming the weights
         # once per 32 tokens through the decode GEMV
         self.use_prefill_tc = _os.environ.get("B200_PREFILL_TC", "1") != "0"
         # verification aid: EVERY forward_inference call (single-token steps too) through the tensor-core GEMM, whose dequant
@@ -204,12 +204,11 @@ class DecodeEngine:
         self._pf = None
         # TP > 1, bs = 1: the all-reduce after wo / w2 is fused into the GEMV kernels (LL push + rank-ordered sum, ll.cuh)
         # instead of 2 NCCL all-reduce kernels per layer
-        # verified at TP = 2 on B200 (813 vs 560 tokens/s with NCCL, logits = TP 1 to one fp16 ulp, profiles/r02k_*); bench.py
-        # re-checks TP = world against TP = 1 before every timed run and falls back to NCCL if the check fails
+        # bench.py re-checks TP = world against TP = 1 before every timed run and falls back to NCCL if the check fails
         self.use_ar_fused = _os.environ.get("B200_TP_LL", "1") != "0"
         self._ar = None
         # L2 prefetch of the head of every CTA region of the NEXT kernel's weights (+ the K/V rows attention will read) by the
-        # producer warps: +2-6 % at bs = 1 once the integer-path GEMV made the step HBM-bound (gpurun_out/r2b_bench.txt)
+        # producer warps (bs = 1: the integer-path GEMV leaves the step HBM-bound)
         self.prefetch_bytes = int(_os_env("B200_PF", "1"))
         self._graphs: Dict[int, tuple] = {}
         self._alloc_buffers()
@@ -650,7 +649,7 @@ class DecodeEngine:
         return a
 
     # ------------------------------------------------------------------ prefill on the tensor cores ----
-    T_PREFILL = 256  # tokens per tcgen05 GEMM launch (TMEM: 128 lanes x 256 fp32 columns per CTA)
+    T_PREFILL = 256  # tokens per wgmma GEMM launch (a CTA holds 128 rows x 256 tokens of fp32 accumulators)
 
     def prefill_tc_supported(self):
         """Per-channel W4 dense LLaMA whose linears tile by 128 output rows: prompts go through b200_prefill_gemm_w4."""
@@ -787,9 +786,11 @@ class DecodeEngine:
     def capture_greedy_loop(self, bsz: int):
         """One CUDA graph = one full greedy decode step with everything resident on the device:
         step(tokens, pos) -> argmax -> tokens, pos += 1   (meta.py:434-448 without the per-token host sync).
-        Returns (graph, launches_per_step). Set self.tokens[:bsz] / self.pos[:bsz] before the first replay."""
+        Returns (graph, launches_per_step). Set self.tokens[:bsz] / self.pos[:bsz] before the first replay; after a replay,
+        self.greedy_logits holds that step's fp32 logits [bsz, vocab] (the graph's static buffer)."""
         def body():
             logits = self._step(bsz, 1, self.cache_seq)
+            self.greedy_logits = logits
             ops.argmax(logits.contiguous(), self.tokens, bsz, logits.shape[-1])
             ops.advance_pos(self.pos, bsz, 1)
         keep_tok, keep_pos = self.tokens.clone(), self.pos.clone()

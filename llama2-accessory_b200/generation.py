@@ -1,4 +1,4 @@
-"""MetaModel.generate / stream_generate / sample_top_p for the B200 engine (SURVEY.md 8f rank 2).
+"""MetaModel.generate / stream_generate / sample_top_p for the decode engine (SURVEY.md 8f rank 2).
 
 Same signatures, argument meaning and results as accessory/model/meta.py:372-565, with the tokenizer handed in
 (`MetaModel` owns one; here it is any object with the reference Tokenizer's methods: ``encode(s, bos, eos)``,

@@ -36,7 +36,7 @@ class ModelArgs:
     max_batch_size: int = 32
     max_seq_len: int = 2048
     rope_scaling: Optional[float] = None
-    # B200 engine knobs (JSON-configurable like every other field, meta.py:33-45)
+    # engine knobs (JSON-configurable like every other field, meta.py:33-45)
     wbits: int = 4
     group_size: int = 0
 

@@ -107,7 +107,7 @@ def decode_step1(args, dataflow=False):
 
 
 def prefill_gemm_w4(lin: PackedLinear, x, out, T):
-    """out[T, N] = x[T, K] . w_hat^T on the tcgen05 tensor cores (per-channel W4, N % 128 == 0)."""
+    """out[T, N] = x[T, K] . w_hat^T on the tensor cores (wgmma) (per-channel W4, N % 128 == 0)."""
     global launch_count
     ls = lin.c_struct()
     _cabi.check(_cabi.lib().b200_prefill_gemm_w4(C.byref(ls), _p(x), _p(out), T, _stream()), "b200_prefill_gemm_w4")

@@ -1,6 +1,6 @@
 """fairscale-style tensor-parallel layers (the API LLaMA2-Accessory imports from
 `fairscale.nn.model_parallel.layers`, llama.py:10-15; signatures as subclassed at
-accessory/model/peft.py:79-89,189-199) re-provided on top of the B200 kernels.
+accessory/model/peft.py:79-89,189-199) re-provided on top of the sm_90a kernels.
 
 Parameters keep the reference's names and shard shapes (Column: [out/TP, in], Row: [out, in/TP],
 Embedding here: full table replicated -- see DESIGN.md), so checkpoints load unchanged.  Inference

@@ -81,8 +81,10 @@ class PortModel:
         self.eps = a.get("norm_eps", 1e-5)
         self.max_seq_len = a.get("max_seq_len", 2048)
         theta = a.get("rope_theta", 10000.0 if kind == "llama" else 1000000.0)
-        self.freqs_cis = precompute_freqs_cis(self.hd, self.max_seq_len * 2, theta, a.get("rope_scaling"))
         self.sd = {k: v.to(dtype) for k, v in sd.items()}
+        # RoPE table, KV cache and mask live where the weights are (the full-size GPU parity tests run the port on the GPU)
+        self.device = next(iter(self.sd.values())).device
+        self.freqs_cis = precompute_freqs_cis(self.hd, self.max_seq_len * 2, theta, a.get("rope_scaling")).to(self.device)
         assert self.H % tp == 0 and self.Hkv % tp == 0
         self.k_cache = self.v_cache = None
         if kind == "mixtral":
@@ -106,8 +108,8 @@ class PortModel:
     def alloc_cache(self, bsz):
         shape = (bsz, self.max_seq_len, self.Hkv, self.hd)
         if self.k_cache is None or self.k_cache[0].shape != shape:
-            self.k_cache = [torch.zeros(shape, dtype=self.dtype) for _ in range(self.L)]
-            self.v_cache = [torch.zeros(shape, dtype=self.dtype) for _ in range(self.L)]
+            self.k_cache = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in range(self.L)]
+            self.v_cache = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in range(self.L)]
 
     # -- blocks ---------------------------------------------------------------------------
     def attention(self, i, x, start_pos, fc, causal):
@@ -125,7 +127,7 @@ class PortModel:
         n_rep = self.H // self.Hkv
         kk = expand_kv(keys, n_rep).transpose(1, 2)
         vv = expand_kv(vals, n_rep).transpose(1, 2)
-        mask = causal_mask(S, keys.shape[1]) if causal else None
+        mask = causal_mask(S, keys.shape[1]).to(self.device) if causal else None
         o = F.scaled_dot_product_attention(q.transpose(1, 2), kk, vv, dropout_p=0.0, attn_mask=mask)
         o = o.transpose(1, 2).contiguous().view(B, S, -1)
         wo = self._w(p + "wo.weight")

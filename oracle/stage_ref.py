@@ -2,9 +2,9 @@
 
 The reference is pure Python, so "building" it is a byte-for-byte copy of the handful of files the path lives in
 (SURVEY.md 8a) from /root/reference into oracle/_ref/accessory/...  oracle/_ref/ is git-ignored (reference sources never
-enter the history) but is NOT gpurun-ignored, so it travels to the GPU box, where /root/reference does not exist:
-tests, smoke() and bench.py's CPU leg / --impl reference can then run the reference itself instead of the port.
-Called by __graft_entry__.build(); idempotent; a no-op where /root/reference is absent (the GPU box uses the staged copy).
+enter the history); a copy of the working tree made after build() carries it to a machine without the reference tree,
+where tests and bench.py's CPU leg / --impl reference can then run the reference itself instead of the port.
+Called by __graft_entry__.build(); idempotent; a no-op where the reference tree is absent.
 """
 import filecmp
 import os

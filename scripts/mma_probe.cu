@@ -1,6 +1,6 @@
-// Issue-rate / latency probe for the legacy warp-level tensor instructions on sm_100a:
+// Issue-rate / latency probe for the legacy warp-level tensor instructions on sm_90a:
 // HMMA.16816.F32 (fp16) vs IMMA.16832.U8.S8 (int8), plus the LOP3 rate, as a function of resident warps per SM
-// and independent accumulator chains per warp.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mma_probe mma_probe.cu
+// and independent accumulator chains per warp.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mma_probe mma_probe.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Per-rank decode-step timing of the SURVEY.md section-8 configurations on ONE B200.
+"""Per-rank decode-step timing of the SURVEY.md section-8 configurations on ONE GPU.
 
 For a TP > 1 configuration this times ONE rank's shard (its weights, its KV heads) with the collectives
 skipped (engine.shard_only) -- the HBM work of a rank, i.e. the per-GPU roofline fraction, NOT the multi-GPU

@@ -1,6 +1,6 @@
-// Standalone HBM streaming probe for sm_100a: how fast can one CTA per SM (or more) pull a big buffer
+// Standalone HBM streaming probe for sm_90a: how fast can one CTA per SM (or more) pull a big buffer
 // through (a) a cp.async.bulk + mbarrier ring with a trivial consumer, (b) plain 128-bit LDG loops?
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o stream_probe scripts/stream_probe.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o stream_probe scripts/stream_probe.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -1,7 +1,7 @@
-// Dependency hand-off cost probe (sm_100a): how long does one "every CTA needs what every CTA just wrote" step take
+// Dependency hand-off cost probe (sm_90a): how long does one "every CTA needs what every CTA just wrote" step take
 //   (a) as a kernel boundary (plain stream order / programmatic dependent launch, inside a CUDA graph),
 //   (b) as a software grid barrier inside one persistent kernel (148 CTAs), idle and while the SMs stream HBM.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o sync_probe sync_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o sync_probe sync_probe.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

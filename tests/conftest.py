@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (H100, sm_90a; run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -31,7 +31,7 @@ _PARITY = {}
 
 
 def record_parity(case, **numbers):
-    """case -> {e16, e32, floor, argmax_agree, ...}; dumped to PARITY_r02.json (repo root and gpurun_out/)."""
+    """case -> {e16, e32, floor, argmax_agree, ...}; dumped to PARITY_r02.json at the repository root (git-ignored)."""
     _PARITY[case] = {k: (float(v) if hasattr(v, "__float__") else v) for k, v in numbers.items()}
 
 
@@ -42,7 +42,7 @@ def pytest_sessionfinish(session, exitstatus):
     out = {"rule": "pass iff |eng-ref16|max <= 1e-3 OR |eng-ref32|max <= RULE_FACTOR * |ref16-ref32|max; "
                    "ref16/ref32 = the unmodified reference (goldens / oracle/_ref) or its bit-pinned port in fp16 / fp32",
            "cases": _PARITY}
-    for d in (ROOT, os.path.join(ROOT, "gpurun_out")):
+    for d in (ROOT,):
         try:
             os.makedirs(d, exist_ok=True)
             path = os.path.join(d, "PARITY_r02.json")

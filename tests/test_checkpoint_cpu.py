@@ -225,34 +225,25 @@ def test_checkpoint_folder_to_engine_and_packed_round_trip(tmp_path, kind, bits,
 
 
 def test_merge_and_inference_agree_with_the_reference_loader(tmp_path):
-    """The UNMODIFIED accessory/util/tensor_parallel.py (imported in the build container, world size 1 shim) reads the
-    same folders: format inference and the merged TP = 1 state dict must agree tensor for tensor."""
-    from oracle import ref_import
-    if not ref_import.available():
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib
-    ref_import.load("llama")
-    tp = importlib.import_module("accessory.util.tensor_parallel")
+    """The UNMODIFIED accessory/util/tensor_parallel.py read the same folders (tests/golden/checkpoint_loader.json, made
+    by oracle/make_golden_checkpoint.py): format inference, shard file names and the merged TP = 1 state dict must agree
+    tensor for tensor, the merged dict loads into the reference Transformer without missing or unexpected weights, and
+    the malformed folders the reference refuses are refused."""
+    from oracle.make_golden_checkpoint import tensor_digest
+    gold = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "checkpoint_loader.json")))
     args, sd = _master("llama")
-    model = ref_import.build_reference_model("llama", dict(args), sd, torch.float16)
-    holder = torch.nn.Module()
-    holder.llma = model
     for fmt in ("consolidated", "meta_ori"):
+        g = gold["formats"][fmt]
         d = str(tmp_path / fmt)
         ck.save_tensor_parallel_shards(sd, d, 2, fmt)
-        assert tuple(tp.infer_checkpoint_format_and_mp_size(d)) == ck.infer_checkpoint_format_and_mp_size(d) == (fmt, 2)
-        assert tp.get_tensor_parallel_shards_file_name(fmt, 2) == ck.get_tensor_parallel_shards_file_name(fmt, 2)
-        import contextlib
-        import io
-        with contextlib.redirect_stdout(io.StringIO()):
-            ref_sd = tp.load_tensor_parallel_model_state_dict(holder, d, fmt)
+        assert list(ck.infer_checkpoint_format_and_mp_size(d)) == g["inferred"] == [fmt, 2]
+        assert list(ck.get_tensor_parallel_shards_file_name(fmt, 2)) == g["shard_file_names"]
         mine = ck.load_tensor_parallel_state_dict(d, 0, 1, fmt)
-        assert set(ref_sd) == set(mine)
-        for k in ref_sd:
-            assert torch.equal(ref_sd[k], mine[k]), k
-        # and it loads into the reference model without missing / unexpected weights
-        res = holder.load_state_dict(ref_sd, strict=False)
-        assert not res.unexpected_keys and all("clip" in k or "rope" in k or "freqs" in k for k in res.missing_keys)
+        assert set(mine) == set(g["merged"])
+        for k in mine:
+            assert tensor_digest(mine[k]) == g["merged"][k], k
+        assert not g["unexpected_after_load"] and all("clip" in k or "rope" in k or "freqs" in k for k in g["missing_after_load"])
+    assert gold["refused"] == ["empty", "mixed"]
     for bad in ("empty", "mixed"):
         d = tmp_path / bad
         d.mkdir()
@@ -261,8 +252,6 @@ def test_merge_and_inference_agree_with_the_reference_loader(tmp_path):
             ck.save_tensor_parallel_shards(sd, str(d), 1, "meta_ori")
         else:
             (d / "x.txt").write_text("x")
-        with pytest.raises(NotImplementedError):
-            tp.infer_checkpoint_format_and_mp_size(str(d))
         with pytest.raises(NotImplementedError):
             ck.infer_checkpoint_format_and_mp_size(str(d))
 

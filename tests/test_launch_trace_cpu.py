@@ -310,7 +310,7 @@ def test_chunked_prompt_covers_every_position_once_in_order(recorder, bsz, seqle
 
 def test_tensor_core_prompt_path_chunks_and_attention_sub_launches(recorder):
     """Prompts > 32 tokens of a per-channel W4 model: one sequence at a time in chunks of <= 256 positions through the
-    tcgen05 GEMM; per chunk and layer: rmsnorm, QKV GEMM, RoPE + cache write, ceil(chunk / 32) attention launches that walk
+    wgmma GEMM; per chunk and layer: rmsnorm, QKV GEMM, RoPE + cache write, ceil(chunk / 32) attention launches that walk
     the chunk's queries in order, wo GEMM, rmsnorm, gate/up GEMM, SiLU*mul, down GEMM; logits from the last position only."""
     eng = _engine(max_seq_len=320)
     assert eng.prefill_tc_supported()

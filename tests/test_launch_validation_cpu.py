@@ -1,7 +1,7 @@
 """CPU (no GPU present): every launch the engine would enqueue for the SURVEY.md section-8 configurations -- at their real
 layer widths, per tensor-parallel rank -- goes through the REAL library's host-side code: argument validation
 (csrc/gemv.cu build_gemv_params, attn.cu, moe.cu, prefill.cu), the integer-path / HMMA dispatch, token-group and ring sizing
-against the B200's shared memory (the library assumes 148 SMs / 227 KB when no device is visible).  Each call must get as far
+against the H100's shared memory (the library assumes 132 SMs / 227 KB when no device is visible).  Each call must get as far
 as its first CUDA runtime call (which fails here with "no driver": rc > 0); a NEGATIVE rc is the library rejecting the
 shapes or pointers the engine handed it -- the failure a first run on hardware would hit.
 
@@ -107,7 +107,7 @@ def test_library_accepts_every_launch_of_the_configuration(validator, name, kind
     if kind == "mixtral":
         assert all(validator.accepted.get(k, 0) > 0 for k in ("b200_moe_route", "b200_moe_expert_ffn", "b200_moe_combine"))
     if bits == 4 and not gs and kind == "llama" and prompt > 32 and bsz == 1:
-        assert validator.accepted.get("b200_prefill_gemm_w4", 0) > 0           # prompts > 32 tokens take the tcgen05 GEMM
+        assert validator.accepted.get("b200_prefill_gemm_w4", 0) > 0           # prompts > 32 tokens take the wgmma GEMM
     if tp > 1 and bsz == 1 and bits == 4 and not gs and kind == "llama":
         assert eng._ar is not None                                             # the fused exchange was armed
 

@@ -118,12 +118,25 @@ def test_unmodified_metamodel_generate_runs_on_the_b200_engine(tmp_path):
     assert ys[-1]["end_of_content"] and ys[-1]["text"] == model.generate([PROMPTS[0]], max_gen_len=5)[0]
 
 
-def test_metamodel_fp16_engine_against_the_reference_goldens(tmp_path):
+def test_metamodel_fp16_engine_against_the_reference_goldens():
     """wbits = 16: the same weights the fp32 goldens of the unmodified reference model were generated from
-    (tests/golden/generate.json); fp16 logits can flip a near-tie, so agreement is counted, not demanded token for token."""
-    meta = _import_meta()
-    model = _metamodel(meta, tmp_path, wbits=16)
-    texts = model.generate(list(PROMPTS), max_gen_len=6)
+    (tests/golden/generate.json); fp16 logits can flip a near-tie, so agreement is counted, not demanded token for token.
+    Self-contained: the drop-in Transformer is built as MetaModel builds it (max_batch_size 32, vocab from the tokenizer)
+    and driven by this repo's statement of MetaModel.generate, which tests/test_generation_cpu.py pins to the same goldens."""
+    args = dict(cases.TINY_LLAMA)
+    cfg = {k: v for k, v in args.items() if k not in ("max_batch_size",)}
+    old = torch.get_default_dtype()
+    torch.set_default_dtype(torch.float16)
+    try:
+        with torch.device("cuda"):
+            model = llama_b200.Transformer(llama_b200.ModelArgs(**cfg, max_batch_size=32, wbits=16))
+    finally:
+        torch.set_default_dtype(old)
+    missing, unexpected = model.load_state_dict({k: v.cuda() for k, v in cases.master_state_dict("llama", args).items()},
+                                                strict=False)
+    assert not missing and not unexpected, (missing, unexpected)
+    model.eval()
+    texts = generation.generate(model, ToyTokenizer(args["vocab_size"], 2), list(PROMPTS), max_gen_len=6, device_loop=False)
     gold = next(c for c in json.load(open(GOLD))["cases"] if c["name"] == "greedy")["texts"]
     first = sum(a.split()[0] == b.split()[0] for a, b in zip(texts, gold))
     n_tok = sum(len(b.split()) for b in gold)

@@ -103,7 +103,7 @@ def test_bit_exact_fake_quant_weight_instance_meets_strict_rule(name):
     rms_floor = float(np.sqrt(np.mean((ref16 - ref32) ** 2)))
     print(f"\n[{name}, bit-exact w_hat instance] |eng-ref16|={e16:.3e} |eng-ref32|={e32:.3e} floor={floor:.3e} rms {rms32:.3e}/{rms_floor:.3e}")
     from conftest import record_parity
-    record_parity(name + "_exact_what_tcgen05", e16=e16, e32=e32, floor=floor, rms32=rms32, rms_floor=rms_floor,
+    record_parity(name + "_exact_what_wgmma", e16=e16, e32=e32, floor=floor, rms32=rms32, rms_floor=rms_floor,
                   strict_pass=bool(e16 <= 1e-3 or e32 <= floor), source="tests/golden (unmodified reference)")
     assert np.isfinite(got).all()
     assert e16 <= 1e-3 or e32 <= 1.1 * floor, (e16, e32, floor)

@@ -1,7 +1,7 @@
 """GPU: full-depth parity on BASELINE.json's headline model -- LLaMA2-7B (32 layers, D = 4096, F = 11008), OmniQuant
 W4A16 per-channel, prefill 128 + 16 single-token decode steps (SURVEY.md 8d schedule) -- against the UNMODIFIED
 reference Transformer (accessory/model/LLM/llama.py, staged under oracle/_ref; the bit-pinned port if absent) run on
-the same B200 in fp32 and in fp16 on the identical fake-quantised weights.  Decode steps go through the persistent
+the same GPU in fp32 and in fp16 on the identical fake-quantised weights.  Decode steps go through the persistent
 whole-step kernel, the prefill through the batched kernels.  Numbers land in PARITY_r02.json.
 """
 import os
@@ -87,8 +87,8 @@ def test_llama2_7b_w4_full_depth_prefill128_decode16():
     record_parity(f"C2_llama2_7b_w4_{n_layers}layers_prefill{plen}_decode{ndec}", e16=e16, e32=e32, floor=floor,
                   rms32=rms32, rms_floor=rms_floor, strict_pass=bool(e16 <= 1e-3 or e32 <= floor),
                   absmax=np.abs(ref32).max(), argmax_agree=agree, argmax_agree_ref16=agree16, rule_factor=RULE_FACTOR,
-                  decode_path=decode_path, prefill_path="tcgen05 GEMM" if eng.prefill_tc_supported() else "GEMV chunks",
-                  source=f"{kind} on the B200 (fp32 / fp16), identical fake-quantised weights")
+                  decode_path=decode_path, prefill_path="wgmma GEMM" if eng.prefill_tc_supported() else "GEMV chunks",
+                  source=f"{kind} on the GPU (fp32 / fp16), identical fake-quantised weights")
     assert np.isfinite(got).all()
     assert (e16 <= 1e-3 or e32 <= RULE_FACTOR * floor
             or (rms32 <= 1.02 * rms_floor and e32 <= 1.25 * floor)), (e16, e32, floor, rms32, rms_floor)

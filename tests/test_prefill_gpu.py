@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 W4A16 prefill GEMM (csrc/prefill.cu) and the prompt path built on it, through the C-ABI.
+"""GPU: the wgmma W4A16 prefill GEMM (csrc/prefill.cu) and the prompt path built on it, through the C-ABI.
 
 GEMM checker: F.linear(x, w_hat) in fp32 with w_hat = fp16(fp16(q - z) * s16) -- the reference's fake-quantised weight,
 which the kernel reproduces bit for bit before the tensor cores multiply it; tolerance = fp16 rounding of the output.
@@ -71,7 +71,7 @@ def test_long_prompt_through_tensor_core_prefill_matches_port(plen):
         e32, e16 = np.abs(got[tc] - ref32).max(), np.abs(got[tc] - ref16).max()
         print(f"\\n[prefill {plen} tc={tc}] |eng-ref16|={e16:.3e} |eng-ref32|={e32:.3e} floor={floor:.3e}")
         from conftest import record_parity
-        record_parity(f"tiny_llama_w4_prefill{plen}_{'tcgen05' if tc else 'gemv_chunks'}", e16=e16, e32=e32, floor=floor,
+        record_parity(f"tiny_llama_w4_prefill{plen}_{'wgmma' if tc else 'gemv_chunks'}", e16=e16, e32=e32, floor=floor,
                       strict_pass=bool(e16 <= 1e-3 or e32 <= floor), source="oracle port fp16 / fp32 on the CPU")
         assert np.isfinite(got[tc]).all()
         assert e16 <= 1e-3 or e32 <= 1.5 * floor, (e16, e32, floor)

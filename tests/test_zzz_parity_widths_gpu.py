@@ -1,10 +1,10 @@
 """GPU: parity at the layer widths of the other BASELINE.json configurations (VERDICT r01 item 2) -- two full blocks +
 lm_head each, against the UNMODIFIED reference Transformer (oracle/_ref; the bit-pinned port if absent) run on the same
-B200 in fp32 and in fp16 on the identical OmniQuant fake-quantised weights:
+GPU in fp32 and in fp16 on the identical OmniQuant fake-quantised weights:
 
   C1 width  LLaMA2-7B    D 4096, 32 heads, F 11008, fp16 weights (no quantiser: BASELINE.json's first configuration, "fp16 single
                          forward seq=128 bs=1"), prompt 128 through the fp16 GEMV family in 32-token chunks + 4 decode steps
-  C3 width  LLaMA2-13B   D 5120, 40 heads, F 13824, W4 per-channel, bs 1, prefill 128 (tcgen05 GEMM) + 8 decode steps
+  C3 width  LLaMA2-13B   D 5120, 40 heads, F 13824, W4 per-channel, bs 1, prefill 128 (wgmma GEMM) + 8 decode steps
                          (integer-path GEMV at K = 5120 / 13824)
   C5 width  LLaMA2-70B   D 8192, 64 query / 8 kv heads (n_rep 8), W3 per-channel (native 3-bit layout), bs 4, prefill 24
                          (chunked GEMV path, token-group split) + 4 batched decode steps.  F = 14336 = the FFN width of
@@ -116,8 +116,8 @@ def test_two_blocks_at_baseline_config_width(name):
     record_parity(name, e16=e16, e32=e32, floor=floor, rms32=rms32, rms_floor=rms_floor,
                   strict_pass=bool(e16 <= 1e-3 or e32 <= floor), absmax=absmax, argmax_agree=agree,
                   argmax_agree_ref16=agree16, rule_factor=RULE_FACTOR, bits=bits, bsz=bsz, prefill=plen, decode=ndec,
-                  prefill_path="tcgen05 GEMM" if (eng.prefill_tc_supported() and plen > 32) else "GEMV chunks",
-                  source=f"{kind} on the B200 (fp32 / fp16), identical fake-quantised weights, 2 blocks + lm_head")
+                  prefill_path="wgmma GEMM" if (eng.prefill_tc_supported() and plen > 32) else "GEMV chunks",
+                  source=f"{kind} on the GPU (fp32 / fp16), identical fake-quantised weights, 2 blocks + lm_head")
     assert (e16 <= 1e-3 or e32 <= RULE_FACTOR * floor or (rms32 <= 1.02 * rms_floor and e32 <= 1.25 * floor)
             or e32 <= 2.05 * ulp), (name, e16, e32, floor, rms32, rms_floor, ulp)
     if clear.any():
