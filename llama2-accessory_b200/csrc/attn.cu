@@ -133,6 +133,10 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     int stage = 0;
     uint32_t par = 0;
     bool waited = false, pf_done = !(p.next_w && p.next_bytes > 0);
+    // the QKV kernel appends the rows of every token of this sequence in the launch, not just row pos[tok]: a prompt chunk
+    // whose positions cross a 32-row tile writes into the tile before the one holding pos[tok] as well
+    int first_new = kv_len - 1;
+    for (int j = brow * p.tps; j < min(p.T, (brow + 1) * p.tps); ++j) first_new = min(first_new, p.pos[j]);
     auto prefetch_next = [&]() {  // pull the next kernel's weights into L2
       pf_done = true;
       const int cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
@@ -142,7 +146,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     for (int i = 0; i < n_tiles; ++i) {
       if (lane == 0) {
         const int s0 = s_begin + i * kTile;
-        const bool dep = !waited && s0 + kTile >= kv_len;  // this tile holds the row the QKV kernel is appending right now
+        const bool dep = !waited && s0 + kTile > first_new;  // this tile holds a row the QKV kernel is appending right now
         // pf_early: the hint goes out as soon as this producer would block (ring full / dependency), not after its last tile
         if (p.pf_early && !pf_done && (i == kStages || dep)) prefetch_next();
         mbar_wait(&empty[stage], par ^ 1);

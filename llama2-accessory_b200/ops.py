@@ -106,9 +106,28 @@ def decode_step1(args, dataflow=False):
     launch_count += 1
 
 
+def _dev(t, name, dtype, numel, on):
+    """The prompt kernels take raw pointers: refuse a tensor they would misread or run past.  `on` is the launch's first
+    fp16 tensor, already checked by _f16 to be a CUDA tensor; every other buffer must live on its device."""
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous() or t.device != on.device:
+        raise ValueError(f"{name} must be a contiguous {dtype} tensor on {on.device}")
+    if t.numel() < numel:
+        raise ValueError(f"{name} has {t.numel()} elements, {numel} needed")
+
+
+def _anchor(t, name):
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name} must be a contiguous CUDA fp16 tensor")
+    _f16(t, name)
+    return t
+
+
 def prefill_gemm_w4(lin: PackedLinear, x, out, T):
     """out[T, N] = x[T, K] . w_hat^T on the tensor cores (wgmma) (per-channel W4, N % 128 == 0)."""
     global launch_count
+    on = _anchor(x, "x")
+    _dev(x, "x", torch.float16, T * lin.K, on)
+    _dev(out, "out", torch.float16, T * lin.N, on)
     ls = lin.c_struct()
     _cabi.check(_cabi.lib().b200_prefill_gemm_w4(C.byref(ls), _p(x), _p(out), T, _stream()), "b200_prefill_gemm_w4")
     launch_count += (T + 255) // 256
@@ -116,13 +135,27 @@ def prefill_gemm_w4(lin: PackedLinear, x, out, T):
 
 def prefill_rmsnorm(resid, delta, h_out, gamma, eps, x_out, T, D):
     global launch_count
+    on = _anchor(resid, "resid")
+    for t, n in ((resid, "resid"), (delta, "delta"), (h_out, "h_out"), (x_out, "x_out")):
+        if t is not None or n in ("resid", "x_out"):
+            _dev(t, n, torch.float16, T * D, on)
+    _dev(gamma, "gamma", torch.float16, D, on)
     _cabi.check(_cabi.lib().b200_prefill_rmsnorm(_p(resid), _p(delta), _p(h_out), _p(gamma), eps, _p(x_out), T, D, _stream()),
                 "b200_prefill_rmsnorm")
     launch_count += 1
 
 
 def prefill_rope_kv(qkv, q_out, kcache, vtcache, rope, pos, T, n_q_rows, n_kv_rows, tokens_per_seq, cache_seq):
+    """Positions are not checked (that would need a device sync): pos[t] < cache_seq and < the rows of `rope`."""
     global launch_count
+    on = _anchor(qkv, "qkv")
+    _dev(qkv, "qkv", torch.float16, T * (n_q_rows + 2 * n_kv_rows), on)
+    _dev(q_out, "q_out", torch.float16, T * n_q_rows, on)
+    n_seq = (T - 1) // max(1, tokens_per_seq) + 1
+    _dev(kcache, "kcache", torch.float16, n_seq * n_kv_rows * cache_seq, on)
+    _dev(vtcache, "vtcache", torch.float16, n_seq * n_kv_rows * cache_seq, on)
+    _dev(rope, "rope", torch.float32, 128, on)
+    _dev(pos, "pos", torch.int32, T, on)
     _cabi.check(_cabi.lib().b200_prefill_rope_kv(_p(qkv), _p(q_out), _p(kcache), _p(vtcache), _p(rope), _p(pos), T, n_q_rows,
                                                  n_kv_rows, tokens_per_seq, cache_seq, _stream()), "b200_prefill_rope_kv")
     launch_count += 1
@@ -130,6 +163,9 @@ def prefill_rope_kv(qkv, q_out, kcache, vtcache, rope, pos, T, n_q_rows, n_kv_ro
 
 def prefill_silu_mul(gu, act, T, F):
     global launch_count
+    on = _anchor(gu, "gu")
+    _dev(gu, "gu", torch.float16, T * 2 * F, on)
+    _dev(act, "act", torch.float16, T * F, on)
     _cabi.check(_cabi.lib().b200_prefill_silu_mul(_p(gu), _p(act), T, F, _stream()), "b200_prefill_silu_mul")
     launch_count += 1
 

@@ -83,7 +83,13 @@ def _np_ptr(a: np.ndarray):
 
 def pack_quantized(q: torch.Tensor, scale: torch.Tensor, zero: torch.Tensor, bits: int, group_size: int,
                    device) -> PackedLinear:
-    """(q uint8 [N,K], scale/zero fp16 [N,G]) -> PackedLinear on `device` (packing runs on the host)."""
+    """(q uint8 [N,K], scale/zero fp16 [N,G]) -> PackedLinear on `device` (packing runs on the host).
+
+    Zero points must be integers with |z| <= 1024: the kernels dequantise (1024 + q) - (1024 + z) in fp16, which is exact
+    only in that range, and a fractional z would round silently."""
+    zf = zero.detach().float()
+    if zf.numel() and (not torch.equal(zf, zf.round()) or float(zf.abs().max()) > 1024):
+        raise ValueError("zero points must be integers with |z| <= 1024 in the packed format")
     lib = _cabi.lib()
     N, K = q.shape
     gs = 0 if (not group_size or group_size >= K) else int(group_size)

@@ -66,6 +66,24 @@ def test_pack_rejects_bad_input():
     assert lib.b200_pack_weight(4, 15, 64, q.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)) < 0
 
 
+@pytest.mark.parametrize("zbad", [7.5, -0.5, 1025.0, -1025.0, 2048.0, float("nan"), float("inf")])
+def test_pack_rejects_zero_points_outside_the_format(zbad):
+    """The prompt GEMM dequantises (1024 + q) - (1024 + z) in fp16: exact only for integer z with |z| <= 1024."""
+    q = torch.zeros(16, 64, dtype=torch.uint8)
+    s = torch.full((16, 1), 1e-3).half()
+    z = torch.full((16, 1), 8.0).half()
+    for zok in (-1024.0, -1023.0, 0.0, 1000.0, 1024.0):  # the edges of the format still pack
+        z[5, 0] = zok
+        quant.pack_quantized(q, s, z, 4, 0, "cpu")
+    z[5, 0] = zbad
+    with pytest.raises(ValueError, match="zero points"):
+        quant.pack_quantized(q, s, z, 4, 0, "cpu")
+    zg = torch.full((16, 2), 8.0).half()  # grouped scales are checked the same way
+    zg[15, 1] = zbad
+    with pytest.raises(ValueError, match="zero points"):
+        quant.pack_quantized(q, s.expand(16, 2).contiguous(), zg, 4, 32, "cpu")
+
+
 # ---- numpy restatement of Codec<BITS>::block -------------------------------------------------------
 def _halves(reg):
     return (reg & 0xFFFF).astype(np.float64), (reg >> 16).astype(np.float64)
