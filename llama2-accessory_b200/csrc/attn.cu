@@ -56,25 +56,12 @@ struct AttnParams {
   int stream_ef; // K/V bulk copies carry the L2 evict_first policy (B200_KV_EF)
   int even;      // keys dealt out to the splits in whole tiles, evenly (B200_ATTN_EVEN)
   int pf_early;  // next-stream L2 prefetch as soon as the producer would block instead of after its last tile
-  int cluster;  // 1: the n_split CTAs of a (token, kv head) form a thread-block cluster and merge through DSMEM
 };
 
 // KV-cache layouts are "shared-memory images" so that one 32-position tile is ONE contiguous 8 KB bulk copy:
 //   K  [B][Hkv][S][128]          with the 16-byte chunk index XOR-swizzled by the row parity: chunk ^ ((s&1)<<2)
 //   V  [B][Hkv][S/32][128][32]   (transposed inside each 32-position block)
 __device__ __forceinline__ int k_swz(int row) { return (row & 1) << 2; }
-
-// thread-block-cluster helpers (distributed shared memory)
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ float ld_dsmem_f32(const float* local_smem_ptr, uint32_t cta_rank) {
-  uint32_t ra;
-  float v;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_smem_ptr)), "r"(cta_rank));
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(ra) : "memory");
-  return v;
-}
 
 __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -295,7 +282,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
 
   const int d = threadIdx.x & 127;  // threads 0..127 <-> 128 output dims (the producer warp only tags along)
   const bool writer = threadIdx.x < 128;
-  float* fin = mml + kAttnWarps * 16 * 2;  // cluster mode: this CTA's merged (o[128], M, L) per head, [16][130]
   for (int h = 0; h < p.n_rep; ++h) {
     float M = -INFINITY;
 #pragma unroll
@@ -312,9 +298,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     if (!writer) continue;
     if (p.n_split == 1) {
       p.out[((size_t)tok * p.Hq + hq) * 128 + d] = __float2half_rn(o / L);
-    } else if (p.cluster) {
-      fin[h * 130 + d] = o;
-      if (d == 0) fin[h * 130 + 128] = M, fin[h * 130 + 129] = L;
     } else {
       p.ws_o[(((size_t)tok * p.Hq + hq) * p.n_split + split) * 128 + d] = o;
       if (d == 0) p.ws_ml[((size_t)tok * p.Hq + hq) * p.n_split + split] = make_float2(M, L);
@@ -325,28 +308,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     if (threadIdx.x == 0) tl_max(p.tl, 3);
     return;
   }
-  if (p.cluster) {
-    // ---- cross-split merge through distributed shared memory: no global round trips, no atomics ----
-    cluster_sync_all();  // every CTA of the cluster has published its (o, M, L)
-    if (split == 0 && writer) {
-      for (int h = 0; h < p.n_rep; ++h) {
-        float M = -INFINITY;
-        for (int r = 0; r < p.n_split; ++r) M = fmaxf(M, ld_dsmem_f32(fin + h * 130 + 128, r));
-        float L = 0.f, o = 0.f;
-        for (int r = 0; r < p.n_split; ++r) {
-          const float mr = ld_dsmem_f32(fin + h * 130 + 128, r);
-          const float f = (mr == -INFINITY) ? 0.f : exp2f(mr - M);
-          L += ld_dsmem_f32(fin + h * 130 + 129, r) * f;
-          o += ld_dsmem_f32(fin + h * 130 + d, r) * f;
-        }
-        p.out[((size_t)tok * p.Hq + kvh * p.n_rep + h) * 128 + d] = __float2half_rn(o / L);
-      }
-    }
-    cluster_sync_all();  // peers keep their shared memory alive until rank 0 has read it
-    if (threadIdx.x == 0) tl_max(p.tl, 3);
-    return;
-  }
-
   // ---- cross-split merge by the last CTA to arrive for this (token, kv head) ----
   __threadfence();
   __syncthreads();
@@ -449,9 +410,9 @@ extern "C" int b200_attn_choose_split(int T, int Hkv, int max_kv_len) {
   const int target = 2 * sm_count();
   int want = target / (T * Hkv);
   const int max_split = (max_kv_len + kChunkAlign - 1) / kChunkAlign;
-  // <= 8 splits merge through distributed shared memory (a portable cluster); more use the workspace merge.  The split
-  // count is not capped at 8: a cluster is only scheduled once 8 CTA slots of one GPC are free at the same time, which
-  // defeats the early start under programmatic dependent launch.
+  // Every split count merges through the workspace (last CTA of a (token, kv head)), never through a thread-block cluster:
+  // a cluster is only scheduled once all its CTA slots in one GPC are free at the same time, which defeats the early start
+  // under programmatic dependent launch (dropping the clusters of 8 CTAs gave 8 % more decode tokens/s at bs = 1 on an H100 SXM).
   const int cap = tune_get("B200_ATTN_MAX_SPLIT", 16);
   want = std::max(1, std::min(want, max_split));
   if (want > cap && T * Hkv * cap >= sm_count()) want = std::max(cap, 1);  // keep >= one CTA per SM when capping
@@ -483,6 +444,11 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
   int chunk = (a->max_kv_len + n_split - 1) / n_split;
   chunk = (chunk + kTile - 1) / kTile * kTile;
   n_split = (a->max_kv_len + chunk - 1) / chunk;
+  // the merge of more than 16 splits stages (m, l) pairs, rescale factors and L of a group in the K/V ring
+  if ((size_t)(a->Hq / a->Hkv) * (n_split * 12 + 4) > (size_t)kStages * kStageBytes) {
+    set_error("attn: too many splits for the merge's shared-memory staging");
+    return B200_E_INVAL;
+  }
   if (n_split > 1 && (!a->ws || !a->counters)) {
     set_error("attn: workspace/counters required when n_split > 1");
     return B200_E_INVAL;
@@ -510,8 +476,6 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
   p.stream_ef = tune_get("B200_KV_EF", 1);
   p.tl = timeline_slot();
   p.tlc = timeline_cta_slot();
-  const int use_cluster = tune_get("B200_ATTN_CLUSTER", 1);
-  p.cluster = (use_cluster && n_split > 1 && n_split <= 8) ? 1 : 0;
 
   const size_t smem = (size_t)kStages * kStageBytes;  // 96 KB ring (also covers the 33 KB merge area)
   static bool configured_dev[16] = {};  // cudaFuncSetAttribute is per device
@@ -531,18 +495,11 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
   cfg.blockDim = dim3(kAttnThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = static_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int na = 0;
   if (a->use_pdl) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (p.cluster) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = n_split;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
     ++na;
   }
   cfg.attrs = attr;

@@ -11,7 +11,7 @@ from llama2_accessory_b200 import _cabi
 from llama2_accessory_b200.engine import DecodeEngine, EngineConfig
 
 DEFAULTS = {"B200_PF_KB": 96, "B200_PF_KV": 1, "B200_SELF_PF_KB": 0, "B200_PF_EARLY": 0, "B200_ATTN_MAX_SPLIT": 16,
-            "B200_GEMV_RING_KB": 128, "B200_QKV_RING_KB": 0, "B200_ATTN_CLUSTER": 1, "B200_ATTN_DEFER_MERGE": 0,
+            "B200_GEMV_RING_KB": 128, "B200_QKV_RING_KB": 0, "B200_ATTN_DEFER_MERGE": 0,
             "B200_EPI_WARPS4": 0, "B200_KEEP_CONST": 1, "B200_CONST_PF": 1, "B200_ATTN_EVEN": 0,
             "B200_G1_HOLD_SLOTS": 0, "B200_G1_DBG": 0, "B200_G1_WARM": 0, "B200_STREAM_EF": 1, "B200_KV_EF": 1}
 SPEC = [
