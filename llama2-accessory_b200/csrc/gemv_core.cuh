@@ -269,7 +269,9 @@ __device__ __forceinline__ uint4 load_h(const GemvParams& p, int tok, int u) {
 // loads of four tokens are in flight together, the raw residual rows are parked in the x buffer itself, one barrier
 // publishes every token's sum of squares, and the normalisation then runs in place out of shared memory.
 // Each thread owns the same elements and every sum is formed in the same order as in the per-token path, so the
-// staged x, csum and xsum are bit-identical to it: results do not depend on the batch size.
+// staged x, csum and xsum are bit-identical to it.  The outputs still depend on the launch's NT class: mma_phase keeps
+// kChunk accumulator sets at NT = 1 (T <= 8) and one at NT = 2 / 4, so a token's y may differ in the last bits between a
+// launch of <= 8 tokens and one of more (tests/test_gemv_batched_moe_gpu.py).
 static __device__ void stage_x_batched(const GemvParams& p, int T, const int* cols, __half* xs, float* csum,
                                        float* xsum, float* scratch, int tid) {
   const int nvec = p.K >> 3;

@@ -21,9 +21,7 @@ References run in float64 on the device.
     launch (RoPE in fp32 without FMA, SiLU in fp32 then fp16, the K / V cache slots) must follow from that fp16 y bit for bit.
   - PDL, L2 prefetches and ring depths change nothing the kernels compute: those cases demand bit identity.
 """
-import contextlib
 import math
-import os
 
 import pytest
 import torch
@@ -31,19 +29,19 @@ import torch
 pytestmark = pytest.mark.gpu
 
 import llama2_accessory_b200 as pkg  # noqa: E402
-from llama2_accessory_b200 import _cabi, kvlayout, ops, quant  # noqa: E402
+from llama2_accessory_b200 import kvlayout, ops, quant  # noqa: E402
 from llama2_accessory_b200.engine import DecodeEngine, EngineConfig, _interleave_w13, rope_table  # noqa: E402
+from oracle.numerics import SENT, fp16_sides as _fp16_sides, nan16, rstd64, tuned as _tuned  # noqa: E402
+from oracle.numerics import x_candidates as _x_candidates  # noqa: E402
 
 DEV = "cuda"
 EPS = 1e-5
 AMB_X = 2.0 ** -18       # relative distance from an fp16 midpoint below which fp16(h * rstd) is ambiguous (see above)
-RSTD_ULPS = 32           # the kernel's fp32 rstd lies within this many fp32 ulps of rstd64 (see above)
 SILU_REL = 2.0 ** -20    # fp32 a / (1 + expf(-a)): expf <= 2 ulp, the add and the division 0.5 ulp each -> <= 3.5u << 16u
 C_ACC16 = 2.0 ** -18     # fp32 tensor-core accumulation of the fp16 HMMA GEMV, relative to |x| . |w|^T (test_prefill_gpu)
 # least fraction of an epilogue launch's fp16 y equal to fp16 of float64 y (best rstd candidate), per channel / grouped.
 # Measured on an H100 80GB HBM3 (400 W limit) over every shape here: 0.998 to 1.0 per channel, 0.977 to 1.0 grouped.
 MIN_EXACT = {False: 0.97, True: 0.9}
-SENT = 0x7E5A            # NaN bit pattern: a sentinel no kernel writes
 SLOT = 16384             # bytes of one weight-ring stage
 
 
@@ -53,25 +51,11 @@ def _built():
 
 
 def _nan16(*shape):
-    return torch.full(shape, SENT, dtype=torch.int16, device=DEV).view(torch.float16)
+    return nan16(*shape, device=DEV)
 
 
 def _gen(seed):
     return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def _fp16_sides(v):
-    """float64 v -> (nearest fp16, the other fp16 neighbour, |v - the midpoint between them|), signed like v."""
-    a = v.abs()
-    _, e = torch.frexp(a)
-    # the fp16 spacing 2^(e - 11), built from its exponent bits: the device exp2 need not return exact powers of two
-    u = ((e.long() - 11 + 1023).clamp_min(1) << 52).view(torch.float64)
-    u = torch.where(a < 2.0 ** -14, torch.full_like(a, 2.0 ** -24), u)
-    lo = torch.floor(a / u) * u
-    mid = lo + u / 2
-    near, alt = torch.where(a < mid, lo, lo + u), torch.where(a < mid, lo + u, lo)
-    sg = torch.where(v < 0, -1.0, 1.0).double()
-    return sg * near, sg * alt, (a - mid).abs()
 
 
 def _acc(y, G):
@@ -116,22 +100,9 @@ def _norm_inputs(K, seed):
     return resid, delta, gamma
 
 
-def _rstd64(h, eps):
-    hd = h.double().reshape(-1)
-    return 1.0 / torch.sqrt(hd.pow(2).mean() + float(torch.tensor(eps, dtype=torch.float32)))
-
-
-def _x_candidates(h, gamma, eps):
-    """[C, K] fp16: x = fp16(fp16(h * rstd) * gamma) for every distinct x that an fp32 rstd within RSTD_ULPS of rstd64 gives."""
-    c = _rstd64(h, eps).float().reshape(1).view(torch.int32)
-    rs = (c + torch.arange(-RSTD_ULPS, RSTD_ULPS + 1, device=DEV, dtype=torch.int32)).view(torch.float32)
-    x = (h.float().reshape(1, -1) * rs[:, None]).half() * gamma.reshape(1, -1)
-    return torch.unique(x.view(torch.int16), dim=0).view(torch.float16)
-
-
 def _x_ref(h, gamma, eps):
     """-> (x from float64 rstd, x with the other rounding of fp16(h * rstd), ambiguous mask)."""
-    v = h.double().reshape(-1) * _rstd64(h, eps)
+    v = h.double().reshape(-1) * rstd64(h, eps)[0]
     near, alt, dist = _fp16_sides(v)
     g = gamma.double().reshape(-1)
     return (near * g).half(), (alt * g).half(), dist <= AMB_X * v.abs()
@@ -322,20 +293,6 @@ def test_gemv1_epilogue_beyond_the_staged_tiles(gs):
 
 
 # ------------------------------------------------------------------ 2. launch arguments that must not change results --
-TUNE_DEFAULTS = {"B200_PF_EARLY": 0, "B200_SELF_PF_KB": 0, "B200_STREAM_EF": 1, "B200_QKV_RING_KB": 0}
-
-
-@contextlib.contextmanager
-def _tuned(name, value):
-    """A b200_tune override lasts for the whole process: put the knob back to what the environment gives."""
-    lib = _cabi.lib()
-    assert lib.b200_tune(name.encode(), value) == 0
-    try:
-        yield
-    finally:
-        lib.b200_tune(name.encode(), int(os.environ.get(name, TUNE_DEFAULTS[name])))
-
-
 def _ndiff(a, b):
     n = 0
     for x, y in zip(a, b):

@@ -13,31 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-
-def kernel_route(logits16, k):
-    """logits16: fp16 [T, E] -> (idx int64 [T, k], weight fp16 [T, k]) following moe.cu line by line (numpy fp32)."""
-    lg = logits16.float().numpy()
-    mx = lg.max(-1, keepdims=True)
-    ex = np.exp((lg - mx).astype(np.float32)).astype(np.float32)
-    den = np.zeros(lg.shape[0], dtype=np.float32)
-    for e in range(lg.shape[1]):                       # sequential fp32 sum over experts, as thread 0 does
-        den = (den + ex[:, e]).astype(np.float32)
-    sc = (ex / den[:, None]).astype(np.float32).astype(np.float16).astype(np.float32)
-    T, E = sc.shape
-    idx = np.zeros((T, k), dtype=np.int64)
-    val = np.zeros((T, k), dtype=np.float32)
-    used = np.zeros((T, E), dtype=bool)
-    for j in range(k):
-        masked = np.where(used, -np.inf, sc)
-        b = masked.argmax(-1)                          # first maximum = lowest index on ties
-        idx[:, j], val[:, j] = b, masked[np.arange(T), b]
-        used[np.arange(T), b] = True
-    s = np.zeros(T, dtype=np.float32)
-    for j in range(k):
-        s = (s + val[:, j]).astype(np.float32)
-    s16 = s.astype(np.float16).astype(np.float32)
-    w = (val / s16[:, None]).astype(np.float32).astype(np.float16)
-    return torch.from_numpy(idx), torch.from_numpy(w)
+from oracle.numerics import kernel_route, kernel_scores
 
 
 @pytest.mark.parametrize("E,k", [(8, 2), (8, 1), (16, 4), (64, 8)])
@@ -65,15 +41,6 @@ def test_routing_model_equals_the_reference_statements(E, k):
     # everywhere: the same SET of experts unless two fp16 scores tie at the boundary or the scores differ in the last bit
     same_set = (idx_k.sort(-1).values == idx_r.sort(-1).values).all(-1)
     assert float(same_set[clear & same_scores].float().mean()) == 1.0
-
-
-def kernel_scores(logits16):
-    lg = logits16.float().numpy()
-    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
-    den = np.zeros(lg.shape[0], dtype=np.float32)
-    for e in range(lg.shape[1]):
-        den = (den + ex[:, e]).astype(np.float32)
-    return (ex / den[:, None]).astype(np.float32).astype(np.float16).astype(np.float32)
 
 
 def test_weights_of_a_token_sum_to_one_within_fp16():
