@@ -255,6 +255,15 @@ int b200_ipc_free(void* own_ptr);
  *   b200_prefill_silu_mul  gu [T][2F] (w1 / w3 interleaved 8 + 8 as for EPI_SILU) -> act [T][F]
  * ---------------------------------------------------------------------------------------------- */
 int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x_fp16, void* out_fp16, int T, b200_stream_t stream);
+/* Grouped MoE form of the same GEMM (Mixtral prompts, mixtral.py:266-294), one launch over a rank's local experts:
+ * for each local expert i (global id e_first + i), for every slot s with slot_expert[s] == e_first + i:
+ *   out[s][0:N] = x[s / src_div][0:K] . w_hat_i^T   (w_hat = fp16(fp16(q - z) * s16), fp32 accumulation, fp16 out)
+ * experts: HOST array of e_count (1..64) per-channel W4 linears with equal N (% 128 == 0) and K (% 64 == 0).
+ * Rows of slots routed elsewhere are not written.  Slots are taken in increasing slot order, 256 per CTA, so every row is
+ * bit-identical to b200_prefill_gemm_w4 on that expert over the gathered rows.  slot_expert: device int32 [n_slots];
+ * x fp16 [(n_slots - 1) / src_div + 1][K]; out fp16 [n_slots][N]. */
+int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_first, int e_count, const int32_t* slot_expert,
+                             int n_slots, int src_div, const void* x_fp16, void* out_fp16, b200_stream_t stream);
 int b200_prefill_rmsnorm(const void* resid, const void* delta, void* h_out, const void* gamma, float eps, void* x_out, int T,
                          int D, b200_stream_t stream);
 int b200_prefill_rope_kv(const void* qkv, void* q_out, void* kcache, void* vtcache, const float* rope, const int32_t* pos, int T,

@@ -118,6 +118,8 @@ SYMBOLS = {
     "b200_ipc_close": (C.c_int, [C.c_void_p]),
     "b200_ipc_free": (C.c_int, [C.c_void_p]),
     "b200_prefill_gemm_w4": (C.c_int, [C.POINTER(Linear), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "b200_prefill_moe_gemm_w4": (C.c_int, [C.POINTER(Linear), C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]),
     "b200_prefill_rmsnorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_int,
                                        C.c_void_p]),
     "b200_prefill_rope_kv": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 5 + [C.c_void_p]),

@@ -24,6 +24,10 @@
 //
 // Pipelines: pk_full (bulk copies -> consumers), b_full (loaders -> consumers), empty (consumers, after the wgmma that read
 // the stage completed -> producer and loaders).
+//
+// Grouped MoE mode (b200_prefill_moe_gemm_w4, Mixtral prompts): the same CTA with routed rows -- the producer streams the
+// CTA's expert, the loaders gather the activation rows of the slots routed to it, the epilogue scatters to those slots
+// (mixtral.py:266-294 runs the experts one at a time the same way: gather, expert, scatter).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -103,9 +107,10 @@ __device__ __forceinline__ uint32_t deq_pair(uint32_t w, __half2 zoff, __half2 s
   return deq2((w >> kShift) & 0x000f000fu, zoff, s2);
 }
 
-template <int NC>
-__global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __grid_constant__ Params p) {
-  extern __shared__ uint8_t smem_raw[];
+// One CTA of the GEMM: 128 output rows x p.T (<= NC * 32) tokens.  kRouted (the grouped MoE GEMM): token t of the CTA is
+// slot rows[t] (shared memory); its activations are row rows[t] / src_div of p.x and its outputs row rows[t] of p.out.
+template <int NC, bool kRouted>
+__device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, const int* rows, int src_div) {
   uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);  // swizzle atoms need 1024-byte alignment
   uint8_t* b_st = smem;                                   // [kStages][32 KB]
   uint8_t* pk_st = b_st + kStages * kBBytes;              // [kStages][4 KB]
@@ -179,7 +184,8 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __gr
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int t = c * 32 + i * 8 + 2 * t4 + e, row = row0 + warp * 16 + g + 8 * h;
-            if (t < p.T && row < p.N) p.out[(size_t)t * p.N + row] = __float2half_rn(acc[c][4 * i + 2 * h + e]);
+            if (t < p.T && row < p.N)
+              p.out[(size_t)(kRouted ? rows[t] : t) * p.N + row] = __float2half_rn(acc[c][4 * i + 2 * h + e]);
           }
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
@@ -211,7 +217,10 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __gr
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           v[u] = make_uint4(0, 0, 0, 0);
-          if (t < p.T) v[u] = *reinterpret_cast<const uint4*>(p.x + (size_t)t * p.K + (size_t)kb * BK + (h + 2 * u) * 8);
+          if (t < p.T) {
+            const int src = kRouted ? rows[t] / src_div : t;
+            v[u] = *reinterpret_cast<const uint4*>(p.x + (size_t)src * p.K + (size_t)kb * BK + (h + 2 * u) * 8);
+          }
         }
         *reinterpret_cast<uint4*>(dst + sw128_offset(t, 0 + h)) = make_uint4(v[0].x, v[1].x, v[2].x, v[3].x);
         *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 + h)) = make_uint4(v[0].y, v[1].y, v[2].y, v[3].y);
@@ -221,6 +230,69 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __gr
       fence_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
       mbar_arrive(&b_full[s]);
     }
+  }
+}
+
+template <int NC>
+__global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __grid_constant__ Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  gemm_w4_cta<NC, false>(p, smem_raw, nullptr, 1);
+}
+
+// ---- grouped MoE GEMM: the same CTA over the slots routed to one expert -------------------------------------------------
+constexpr int kMaxMoeExperts = 64;  // the router's limit (moe.cu kMaxExperts)
+
+struct MoeParams {
+  const int32_t* slot_expert;  // [n_slots] global expert id of every slot
+  const __half* x;             // [n_slots / src_div rows][K]
+  __half* out;                 // [n_slots][N]
+  int N, K, n_slots, src_div, e_first;
+  const uint8_t* qw[kMaxMoeExperts];
+  const __half2* sz[kMaxMoeExperts];
+};
+
+// grid (N / 128, e_count, ceil(n_slots / 256)): CTA (x, i, b) owns output rows [128 x, 128 x + 128) of expert e_first + i for
+// entries [256 b, 256 b + 256) of that expert's slot list (its slots in increasing order).  Every CTA scans slot_expert
+// itself (n_slots int32, L2-resident), so the launch needs no workspace, atomics or index-building pass; a CTA with no
+// entries exits before it issues any copy.
+__global__ void __launch_bounds__(kThreads, 1) prefill_moe_gemm_w4_kernel(const __grid_constant__ MoeParams mp) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ int rows[kMaxT];
+  __shared__ int warp_hits[kThreads / 32];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int expert = mp.e_first + blockIdx.y, lo = blockIdx.z * kMaxT;
+  int found = 0;  // list entries in the slots scanned so far (CTA-uniform)
+  for (int s0 = 0; s0 < mp.n_slots && found < lo + kMaxT; s0 += kThreads) {
+    const int s = s0 + tid;
+    const bool hit = s < mp.n_slots && mp.slot_expert[s] == expert;
+    const uint32_t m = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) warp_hits[warp] = __popc(m);
+    __syncthreads();
+    int idx = found + __popc(m & ((1u << lane) - 1u));
+    for (int w = 0; w < kThreads / 32; ++w) {
+      const int c = warp_hits[w];
+      idx += w < warp ? c : 0;
+      found += c;
+    }
+    if (hit && idx >= lo && idx < lo + kMaxT) rows[idx - lo] = s;
+    __syncthreads();  // warp_hits is rewritten by the next round; rows is complete after the last one
+  }
+  const int n = min(found - lo, kMaxT);
+  if (n <= 0) return;
+  Params p;
+  p.qw = mp.qw[blockIdx.y];
+  p.sz = mp.sz[blockIdx.y];
+  p.x = mp.x;
+  p.out = mp.out;
+  p.N = mp.N, p.K = mp.K, p.KB = mp.K / BK, p.T = n;
+  switch ((n + kNChunk - 1) / kNChunk) {  // the accumulator count is a compile-time NC, as in the dense launches
+#define B200_NC(NC)                                          \
+  case NC:                                                   \
+    p.T_pad = NC * kNChunk;                                  \
+    gemm_w4_cta<NC, true>(p, smem_raw, rows, mp.src_div);    \
+    break;
+    B200_NC(1) B200_NC(2) B200_NC(3) B200_NC(4) B200_NC(5) B200_NC(6) B200_NC(7) B200_NC(8)
+#undef B200_NC
   }
 }
 
@@ -348,6 +420,60 @@ extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, voi
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error(std::string("prefill_gemm_w4: launch: ") + cudaGetErrorString(e));
+    return (int)e;
+  }
+  return 0;
+}
+
+extern "C" int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_first, int e_count, const int32_t* slot_expert,
+                                        int n_slots, int src_div, const void* x, void* out, b200_stream_t stream) {
+  using namespace b200::prefill;
+  if (!experts || !slot_expert || !x || !out) {
+    set_error("prefill_moe_gemm_w4: null pointer");
+    return B200_E_INVAL;
+  }
+  if (e_count < 1 || n_slots < 1 || src_div < 1) {
+    set_error("prefill_moe_gemm_w4: e_count, n_slots and src_div must be >= 1");
+    return B200_E_INVAL;
+  }
+  if (e_count > kMaxMoeExperts) {
+    set_error("prefill_moe_gemm_w4: more than 64 experts in one launch");
+    return B200_E_UNSUPPORTED;
+  }
+  MoeParams mp = {};
+  mp.N = experts[0].N, mp.K = experts[0].K;
+  for (int i = 0; i < e_count; ++i) {
+    const b200_linear_t& l = experts[i];
+    if (l.bits != 4 || (l.group_size > 0 && l.group_size < l.K) || l.N != mp.N || l.K != mp.K || (l.N % BM) || (l.K % BK) ||
+        l.N < BM || l.K < BK || !l.qweight || !l.scales) {
+      set_error("prefill_moe_gemm_w4: per-channel W4 experts of equal N % 128 == 0 and K % 64 == 0 required");
+      return B200_E_UNSUPPORTED;
+    }
+    mp.qw[i] = static_cast<const uint8_t*>(l.qweight);
+    mp.sz[i] = static_cast<const __half2*>(l.scales);
+  }
+  mp.slot_expert = slot_expert;
+  mp.x = static_cast<const __half*>(x);
+  mp.out = static_cast<__half*>(out);
+  mp.n_slots = n_slots, mp.src_div = src_div, mp.e_first = e_first;
+  static bool configured[16] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  dev &= 15;
+  if (!configured[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(prefill_moe_gemm_w4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      set_error(std::string("prefill_moe_gemm_w4: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
+      return (int)e;
+    }
+    configured[dev] = true;
+  }
+  const dim3 grid(mp.N / BM, e_count, (n_slots + kMaxT - 1) / kMaxT);
+  prefill_moe_gemm_w4_kernel<<<grid, kThreads, kSmemBytes, static_cast<cudaStream_t>(stream)>>>(mp);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error(std::string("prefill_moe_gemm_w4: launch: ") + cudaGetErrorString(e));
     return (int)e;
   }
   return 0;

@@ -652,22 +652,28 @@ class DecodeEngine:
     T_PREFILL = 256  # tokens per wgmma GEMM launch (a CTA holds 128 rows x 256 tokens of fp32 accumulators)
 
     def prefill_tc_supported(self):
-        """Per-channel W4 dense LLaMA whose linears tile by 128 output rows: prompts go through b200_prefill_gemm_w4."""
+        """Per-channel W4 dense LLaMA or Mixtral whose linears (experts included) tile by 128 output rows: prompts go through
+        b200_prefill_gemm_w4 and, for the experts, b200_prefill_moe_gemm_w4."""
         c = self.cfg
-        if not self.use_prefill_tc or c.kind != "llama" or c.bits != 4 or c.group_size or self.shard_only:
+        if not self.use_prefill_tc or c.kind not in ("llama", "mixtral") or c.bits != 4 or c.group_size or self.shard_only:
             return False
-        return all(pl.N % 128 == 0 and pl.K % 64 == 0
-                   for pl in (self.layers[0].wqkv, self.layers[0].wo, self.layers[0].w13, self.layers[0].w2))
+        lw = self.layers[0]
+        lins = (lw.wqkv, lw.wo, lw.w13, lw.w2) if c.kind == "llama" else (lw.wqkv, lw.wo, *lw.e_w13, *lw.e_w2)
+        return all(pl.N % 128 == 0 and pl.K % 64 == 0 for pl in lins)
 
     def _prefill_bufs(self):
         if self._pf is None:
             c, dev, f16 = self.cfg, self.device, torch.float16
             T = self.T_PREFILL
             z = lambda *s: torch.zeros(*s, dtype=f16, device=dev)  # noqa: E731
+            # Mixtral: the FFN works on T x top-k slot rows (gate/up output, activations, expert outputs per slot)
+            ns = T * c.experts_per_tok if c.kind == "mixtral" else T
             self._pf = dict(h=[z(T, c.dim), z(T, c.dim)], x=z(T, c.dim), qkv=z(T, (self.Hq + 2 * self.Hkv) * 128),
-                            q=z(T, self.Hq * 128), attn=z(T, self.Hq * 128), o=z(T, c.dim), gu=z(T, 2 * self.F),
-                            act=z(T, self.F), f=z(T, c.dim), pos=torch.zeros(T, dtype=torch.int32, device=dev),
+                            q=z(T, self.Hq * 128), attn=z(T, self.Hq * 128), o=z(T, c.dim), gu=z(ns, 2 * self.F),
+                            act=z(ns, self.F), f=z(T, c.dim), pos=torch.zeros(T, dtype=torch.int32, device=dev),
                             tok=torch.zeros(T, dtype=torch.int64, device=dev))
+            if c.kind == "mixtral":
+                self._pf.update(slot_w=z(ns), slot_e=torch.zeros(ns, dtype=torch.int32, device=dev), y_slot=z(ns, c.dim))
         return self._pf
 
     def _prefill_chunk_tc(self, tokens, pos, tokens_per_seq, row0, max_kv_len, want_rows):
@@ -702,11 +708,28 @@ class DecodeEngine:
                                 counters=self.counters, n_split=n_split, use_pdl=False)
             ops.prefill_gemm_w4(lw.wo, b["attn"], b["o"], T)
             self._allreduce(b["o"], T)
-            ops.prefill_rmsnorm(b["h"][cur], b["o"], b["h"][1 - cur], lw.ffn_norm, c.norm_eps, b["x"], T, c.dim)
-            cur = 1 - cur
-            ops.prefill_gemm_w4(lw.w13, b["x"], b["gu"], T)
-            ops.prefill_silu_mul(b["gu"], b["act"], T, self.F)
-            ops.prefill_gemm_w4(lw.w2, b["act"], b["f"], T)
+            if c.kind == "llama":
+                ops.prefill_rmsnorm(b["h"][cur], b["o"], b["h"][1 - cur], lw.ffn_norm, c.norm_eps, b["x"], T, c.dim)
+                cur = 1 - cur
+                ops.prefill_gemm_w4(lw.w13, b["x"], b["gu"], T)
+                ops.prefill_silu_mul(b["gu"], b["act"], T, self.F)
+                ops.prefill_gemm_w4(lw.w2, b["act"], b["f"], T)
+            else:
+                # MoE block (mixtral.py:266-294): route the T tokens to T x top-k slots, run every local expert over its
+                # slots in one grouped GEMM per projection, combine the slots' outputs per token
+                k = c.experts_per_tok
+                ns, fe = T * k, lw.e_w2[0].K  # fe: the experts' own FFN width (they are not padded to self.F)
+                ops.moe_route(T=T, D=c.dim, E=c.num_experts, topk=k, resid=b["h"][cur], delta=b["o"], h_out=b["h"][1 - cur],
+                              gamma=lw.ffn_norm, eps=c.norm_eps, gate_w=lw.gate, xn_out=b["x"], slot_weight=b["slot_w"],
+                              slot_expert=b["slot_e"])
+                cur = 1 - cur
+                ops.prefill_moe_gemm_w4(lw.e_w13, b["x"], b["gu"], slot_expert=b["slot_e"], n_slots=ns, src_div=k,
+                                        e_first=self.e_first)
+                ops.prefill_silu_mul(b["gu"], b["act"], ns, fe)
+                ops.prefill_moe_gemm_w4(lw.e_w2, b["act"], b["y_slot"], slot_expert=b["slot_e"], n_slots=ns, src_div=1,
+                                        e_first=self.e_first)
+                ops.moe_combine(b["y_slot"], b["slot_w"], b["slot_e"], b["f"], T=T, D=c.dim, topk=k, e_first=self.e_first,
+                                e_count=self.E_loc)
             self._allreduce(b["f"], T)
             delta = b["f"]
         if want_rows is None:

@@ -133,6 +133,23 @@ def prefill_gemm_w4(lin: PackedLinear, x, out, T):
     launch_count += (T + 255) // 256
 
 
+def prefill_moe_gemm_w4(experts, x, out, *, slot_expert, n_slots, src_div, e_first):
+    """Grouped GEMM over the local experts (list of PackedLinear, global ids e_first ..): out[s] = x[s // src_div] . w_hat^T
+    for every slot s routed to one of them; other rows of out are not written."""
+    global launch_count
+    on = _anchor(x, "x")
+    if not experts:
+        raise ValueError("experts must be a non-empty list of PackedLinear")
+    N, K = experts[0].N, experts[0].K
+    _dev(x, "x", torch.float16, ((n_slots - 1) // max(1, src_div) + 1) * K, on)
+    _dev(out, "out", torch.float16, n_slots * N, on)
+    _dev(slot_expert, "slot_expert", torch.int32, n_slots, on)
+    arr = (_cabi.Linear * len(experts))(*[w.c_struct() for w in experts])
+    _cabi.check(_cabi.lib().b200_prefill_moe_gemm_w4(arr, e_first, len(experts), _p(slot_expert), n_slots, src_div, _p(x),
+                                                     _p(out), _stream()), "b200_prefill_moe_gemm_w4")
+    launch_count += 1
+
+
 def prefill_rmsnorm(resid, delta, h_out, gamma, eps, x_out, T, D):
     global launch_count
     on = _anchor(resid, "resid")
