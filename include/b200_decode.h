@@ -247,8 +247,10 @@ int b200_ipc_free(void* own_ptr);
 /* ------------------------------------------------------------------------------------------------
  * Prefill (prompt) path on the Hopper tensor cores: out[T, N] = x[T, K] . w_hat[N, K]^T with
  * w_hat = fp16(fp16(q - z) * s16), the reference's fake-quantised weight reproduced bit for bit, fp32 accumulation in
- * registers (wgmma, M = 128 weight rows per CTA, N = up to 256 tokens per launch, K = 64 per pipeline stage).
- * Replaces F.linear at M = prompt tokens (quant.py:18-46) for per-channel W4 linears with N % 128 == 0, K % 64 == 0.
+ * registers (wgmma, M = 128 weight rows per CTA, N = up to 256 tokens per launch, K = 64 per pipeline stage; 80 for W3).
+ * Replaces F.linear at M = prompt tokens (quant.py:18-46) for per-channel W4 (bits 4) and W3 (bits 3) linears and fp16
+ * linears (bits 16, w_hat = w) with N % 128 == 0 and K % 64 == 0 (W3: K % 16 == 0).  Group scales, W2 and any other
+ * width return B200_E_UNSUPPORTED.
  * The elementwise kernels are the unfused forms of the decode GEMV's prologue / epilogues for T-token chunks:
  *   b200_prefill_rmsnorm   h = resid (+ delta) -> h_out (may be NULL); x = fp16(h * rsqrt(mean h^2 + eps)) * gamma
  *   b200_prefill_rope_kv   qkv [T][n_q + 2 n_kv] -> RoPE; q -> q_out [T][n_q]; k, v -> cache rows pos[t] (llama.py:151-168)

@@ -1,33 +1,40 @@
-// W4A16 prefill GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers) and the elementwise kernels
-// around it; replaces F.linear at M = prompt tokens (accessory/util/quant.py:18-46, llama.py:276-288) for prompts longer
-// than one 32-token chunk of the decode GEMV.
+// Prompt GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers) for per-channel W4 / W3 and fp16 linears,
+// and the elementwise kernels around it; replaces F.linear at M = prompt tokens (accessory/util/quant.py:18-46,
+// llama.py:276-288) for prompts longer than one 32-token chunk of the decode GEMV.
 //
 // GEMM:   out[T, N] = x[T, K] . w_hat[N, K]^T
 //   w_hat = fp16(fp16(q - z) * s16)  -- the reference's fake-quantised weight, reproduced bit for bit, so the prefill
-//   logits follow F.linear(x, w_hat) with fp32 accumulation (accessory/util/quant.py:18-46 + SURVEY.md 8c).
+//   logits follow F.linear(x, w_hat) with fp32 accumulation (accessory/util/quant.py:18-46 + SURVEY.md 8c).  For fp16
+//   linears w_hat is the weight itself.
 //
 // One CTA owns 128 output rows (eight 16-row tiles of the packed decode format, DESIGN.md section 3) and up to 256
-// tokens.  D[rows x tokens] = A . B^T with A = dequantised weights (wgmma register operand), B = activations [T_pad x 64]
-// fp16 per k-block in shared memory (K-major, 128-byte swizzle), D in registers (fp32).
+// tokens.  D[rows x tokens] = A . B^T with A = dequantised weights (wgmma register operand), B = activations [T_pad x kK]
+// fp16 per pipeline stage in shared memory (K-major), D in registers (fp32).
 //
 // Warp roles (12 warps, three warpgroups; setmaxnreg moves registers from the third to the accumulators of the first two):
-//   0..7   two consumer warpgroups; warp w owns the 16-row tile w.  Per k-block: ld.shared of its packed uint4, dequant
-//          into four m64k16 A fragments, 4 x NC wgmma m64n32k16 (NC = T_pad / 32), wait; fp16 stores at the end
-//   8      producer: packed W4 k-blocks HBM -> smem (8 bulk copies of 512 B per k-block, mbarrier expect_tx)
-//   9..10  activation loaders: x[T][kb*64 .. +64] -> B stage, k permuted to the order of the packed fragments (below)
+//   0..7   two consumer warpgroups; warp w owns the 16-row tile w.  Per stage: ld.shared of its packed uint4(s), dequant
+//          into kSteps m64k16 A fragments, kSteps x NC wgmma m64n32k16 (NC = T_pad / 32), wait; fp16 stores at the end
+//   8      producer: packed weights HBM -> smem (8 bulk copies of one tile's stage bytes, mbarrier expect_tx)
+//   9..10  activation loaders: x[T][stage k range] -> B stage, k permuted to the order of the packed fragments (below)
 //   11     idle
 //
-// k order inside a 64-wide k-block.  Lane (g, t) of a packed tile holds rows g, g+8 at physical k 16t .. 16t+15 (four
-// words: row g / g+8 x k 16t+0..7 / 16t+8..15), so the A fragment of k-step j is built from its own registers when
-// logical k 16j + 8h + 2t + e (the fragment position, e = 0, 1) stands for physical k 16t + 8h + 2j + e.  The loaders
-// store the activations in that logical order; the k-sum is the same sum.
+// Per codec (pack.cpp), one stage holds:
+//   W4   one 64-k block: lane (g, t) of a packed tile holds rows g, g+8 at physical k 16t .. 16t+15 (four words: row g /
+//        g+8 x k 16t+0..7 / 16t+8..15).  The A fragment of k-step j is built from its own registers when logical k
+//        16j + 8h + 2t + e (the fragment position, e = 0, 1) stands for physical k 16t + 8h + 2j + e.
+//   W3   one 80-k block (5 k-steps): the lane holds k 20t .. 20t+19 (words: row g / g+8 x k 20t+0..9 / 20t+10..19);
+//        logical k 16j + 8h + 2t + e stands for physical k 20t + 10h + 2j + e.  K need not be a multiple of 80: the
+//        packer pads the last block with q = 0 (w_hat = -z s != 0), so the loaders write zero activations at k >= K.
+//   fp16 four 16-k blocks: the lane's uint4 of block j is already the A fragment of k-step j when logical k
+//        16j + 8h + 2t + e stands for physical k 16j + 4t + 2h + e.
+// The loaders store the activations in that logical order; the k-sum is the same sum.
 //
 // Pipelines: pk_full (bulk copies -> consumers), b_full (loaders -> consumers), empty (consumers, after the wgmma that read
 // the stage completed -> producer and loaders).
 //
-// Grouped MoE mode (b200_prefill_moe_gemm_w4, Mixtral prompts): the same CTA with routed rows -- the producer streams the
-// CTA's expert, the loaders gather the activation rows of the slots routed to it, the epilogue scatters to those slots
-// (mixtral.py:266-294 runs the experts one at a time the same way: gather, expert, scatter).
+// Grouped MoE mode (b200_prefill_moe_gemm_w4, Mixtral prompts, W4 only): the same CTA with routed rows -- the producer
+// streams the CTA's expert, the loaders gather the activation rows of the slots routed to it, the epilogue scatters to
+// those slots (mixtral.py:266-294 runs the experts one at a time the same way: gather, expert, scatter).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,16 +52,28 @@ namespace prefill {
 constexpr int BM = 128, BK = 64, kStages = 4, kMaxT = 256, kNChunk = 32;
 constexpr int kConsumerWarps = 8;
 constexpr int kThreads = (kConsumerWarps + 4) * 32;
-constexpr int kBBytes = kMaxT * BK * 2;     // 32 KB
-constexpr int kPackedBytes = 8 * 512;       // 4 KB: one k-block of eight 16-row tiles
-constexpr size_t kSmemBytes = (size_t)kStages * (kBBytes + kPackedBytes) + 3 * kStages * 8 + 1024;
+
+enum class Codec { W4, W3, F16 };
+
+// One pipeline stage of a codec: kK logical k (kSteps wgmma k-steps), kTileBytes packed bytes of one 16-row tile (contiguous
+// in the tile-major layout), kBBytes of activations for 256 tokens.  Four stages fit the 227 KB of an H100 SM for all three:
+// W4 4 x (32 + 4) KB, W3 4 x (40 + 4) KB, fp16 4 x (32 + 16) KB.
+template <Codec C>
+struct Stage {
+  static constexpr int kK = C == Codec::W3 ? 80 : 64;
+  static constexpr int kSteps = kK / 16;
+  static constexpr int kTileBytes = C == Codec::F16 ? 4 * 512 : 512;
+  static constexpr int kPackedBytes = 8 * kTileBytes;
+  static constexpr int kBBytes = kMaxT * kK * 2;
+  static constexpr size_t kSmemBytes = (size_t)kStages * (kBBytes + kPackedBytes) + 3 * kStages * 8 + 1024;
+};
 
 struct Params {
-  const uint8_t* qw;     // packed W4, tile-major (b200_pack_weight)
-  const __half2* sz;     // per-channel (s, z) [N]
+  const uint8_t* qw;     // packed weights, tile-major (b200_pack_weight / b200_pack_f16)
+  const __half2* sz;     // per-channel (s, z) [N]; unused for fp16
   const __half* x;       // [T][K]
   __half* out;           // [T][N]
-  int N, K, KB, T, T_pad;  // T_pad = NC * 32 >= T, <= 256
+  int N, K, KB, T, T_pad;  // KB: pipeline stages over K; T_pad = NC * 32 >= T, <= 256
 };
 
 // K-major, SWIZZLE_128B canonical layout of a [rows x 64] fp16 tile: 8-row groups of 1024 B, 16-byte chunk c of row r
@@ -72,6 +91,21 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
   d |= (uint64_t)1 << 62;
+  return d;
+}
+
+// W3 stages are 80 k wide, which no 64-k swizzle atom tiles: K-major without swizzle (layout type 0), one column of
+// 8 x 16-byte core matrices per 16-k step.  Core matrix (8-row group r8, k half h) of step j at
+// j * 8192 + r8 * 256 + h * 128, its row r at + 16 r: LBO = 128 B between the two k halves, SBO = 256 B between 8-row groups.
+constexpr int kW3StepBytes = kMaxT * 16 * 2;
+__device__ __forceinline__ uint32_t w3_offset(int row, int step, int half) {
+  return (uint32_t)(step * kW3StepBytes + (row >> 3) * 256 + half * 128 + (row & 7) * 16);
+}
+__device__ __forceinline__ uint64_t make_desc_w3(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3ffff) >> 4);
+  d |= (uint64_t)(128 >> 4) << 16;
+  d |= (uint64_t)(256 >> 4) << 32;
   return d;
 }
 
@@ -106,14 +140,23 @@ __device__ __forceinline__ uint32_t deq_pair(uint32_t w, __half2 zoff, __half2 s
   constexpr int kShift = (J & 1) * 8 + (J >> 1) * 4;
   return deq2((w >> kShift) & 0x000f000fu, zoff, s2);
 }
+// k pair 2j, 2j+1 of one packed W3 u32 (10 consecutive k of one row, pack.cpp kW3Base: pair j's even element in the
+// 3-bit field kW3Base[j] of the low half-word, its odd element in the same field of the high half-word)
+template <int J>
+__device__ __forceinline__ uint32_t deq_pair_w3(uint32_t w, __half2 zoff, __half2 s2) {
+  constexpr int kBase[5] = {0, 3, 1, 4, 2};
+  return deq2((w >> (3 * kBase[J])) & 0x00070007u, zoff, s2);
+}
 
 // One CTA of the GEMM: 128 output rows x p.T (<= NC * 32) tokens.  kRouted (the grouped MoE GEMM): token t of the CTA is
 // slot rows[t] (shared memory); its activations are row rows[t] / src_div of p.x and its outputs row rows[t] of p.out.
-template <int NC, bool kRouted>
-__device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, const int* rows, int src_div) {
+template <Codec C, int NC, bool kRouted>
+__device__ __forceinline__ void gemm_cta(const Params& p, uint8_t* smem_raw, const int* rows, int src_div) {
+  using S = Stage<C>;
+  constexpr int kBBytes = S::kBBytes, kPackedBytes = S::kPackedBytes;
   uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);  // swizzle atoms need 1024-byte alignment
-  uint8_t* b_st = smem;                                   // [kStages][32 KB]
-  uint8_t* pk_st = b_st + kStages * kBBytes;              // [kStages][4 KB]
+  uint8_t* b_st = smem;                                   // [kStages][kBBytes]
+  uint8_t* pk_st = b_st + kStages * kBBytes;              // [kStages][kPackedBytes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(pk_st + kStages * kPackedBytes);
   uint64_t* pk_full = bars;                 // [kStages] producer -> consumers (tx bytes)
   uint64_t* b_full = pk_full + kStages;     // [kStages] loaders (64) -> consumers
@@ -137,11 +180,14 @@ __device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, 
     // ---------------- consumers: dequant -> wgmma, then the fp16 epilogue ----------------
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     const int g = lane >> 2, t4 = lane & 3;
-    const __half2 sz_lo = p.sz[row0 + warp * 16 + g], sz_hi = p.sz[row0 + warp * 16 + g + 8];
-    const __half2 s_lo = __half2half2(__low2half(sz_lo)), s_hi = __half2half2(__low2half(sz_hi));
-    // 1024 + z: exact for |z| <= 1024
-    const __half2 z_lo = __hadd2(__half2half2(__high2half(sz_lo)), __float2half2_rn(1024.f));
-    const __half2 z_hi = __hadd2(__half2half2(__high2half(sz_hi)), __float2half2_rn(1024.f));
+    __half2 s_lo, s_hi, z_lo, z_hi;
+    if constexpr (C != Codec::F16) {
+      const __half2 sz_lo = p.sz[row0 + warp * 16 + g], sz_hi = p.sz[row0 + warp * 16 + g + 8];
+      s_lo = __half2half2(__low2half(sz_lo)), s_hi = __half2half2(__low2half(sz_hi));
+      // 1024 + z: exact for |z| <= 1024
+      z_lo = __hadd2(__half2half2(__high2half(sz_lo)), __float2half2_rn(1024.f));
+      z_hi = __hadd2(__half2half2(__high2half(sz_hi)), __float2half2_rn(1024.f));
+    }
     float acc[NC][16];
 #pragma unroll
     for (int c = 0; c < NC; ++c)
@@ -151,24 +197,46 @@ __device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, 
       const int s = kb % kStages;
       const uint32_t par = (kb / kStages) & 1;
       mbar_wait(&pk_full[s], par);
-      const uint4 w = lds_v4(pk_st + s * kPackedBytes + warp * 512 + lane * 16);
-      // words: [0] row g, k 16t4 + 0..7; [1] row g+8, same k; [2] row g, k 16t4 + 8..15; [3] row g+8, same k
-      uint32_t a[4][4];
+      uint32_t a[S::kSteps][4];
+      if constexpr (C == Codec::F16) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint4 w = lds_v4(pk_st + s * kPackedBytes + warp * S::kTileBytes + j * 512 + lane * 16);
+          a[j][0] = w.x, a[j][1] = w.y, a[j][2] = w.z, a[j][3] = w.w;
+        }
+      } else {
+        const uint4 w = lds_v4(pk_st + s * kPackedBytes + warp * 512 + lane * 16);
+        // words: [0] row g, first half of the lane's k run; [1] row g+8, same k; [2] row g, second half; [3] row g+8
+        if constexpr (C == Codec::W4) {
 #define B200_FRAG(J)                               \
   a[J][0] = deq_pair<J>(w.x, z_lo, s_lo);          \
   a[J][1] = deq_pair<J>(w.y, z_hi, s_hi);          \
   a[J][2] = deq_pair<J>(w.z, z_lo, s_lo);          \
   a[J][3] = deq_pair<J>(w.w, z_hi, s_hi);
-      B200_FRAG(0) B200_FRAG(1) B200_FRAG(2) B200_FRAG(3)
+          B200_FRAG(0) B200_FRAG(1) B200_FRAG(2) B200_FRAG(3)
 #undef B200_FRAG
+        } else {
+#define B200_FRAG(J)                               \
+  a[J][0] = deq_pair_w3<J>(w.x, z_lo, s_lo);       \
+  a[J][1] = deq_pair_w3<J>(w.y, z_hi, s_hi);       \
+  a[J][2] = deq_pair_w3<J>(w.z, z_lo, s_lo);       \
+  a[J][3] = deq_pair_w3<J>(w.w, z_hi, s_hi);
+          B200_FRAG(0) B200_FRAG(1) B200_FRAG(2) B200_FRAG(3) B200_FRAG(4)
+#undef B200_FRAG
+        }
+      }
       mbar_wait(&b_full[s], par);
       const uint32_t b0 = smem_u32(b_st + s * kBBytes);
       wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < BK / 16; ++j)  // +32 bytes per K = 16 step inside the 128-byte swizzle atom
+      for (int j = 0; j < S::kSteps; ++j)
 #pragma unroll
-        for (int c = 0; c < NC; ++c)     // +32 rows (4 swizzle atoms of 8 rows) per n-chunk
-          wgmma_m64n32k16(acc[c], a[j], make_desc(b0 + c * 4096 + j * 32));
+        for (int c = 0; c < NC; ++c) {   // +32 rows per n-chunk
+          if constexpr (C == Codec::W3)
+            wgmma_m64n32k16(acc[c], a[j], make_desc_w3(b0 + j * kW3StepBytes + c * 1024));
+          else  // +32 bytes per K = 16 step inside the 128-byte swizzle atom, 4 swizzle atoms of 8 rows per n-chunk
+            wgmma_m64n32k16(acc[c], a[j], make_desc(b0 + c * 4096 + j * 32));
+        }
       wgmma_commit();
       wgmma_wait_all();
       __syncwarp();
@@ -199,33 +267,68 @@ __device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, 
         mbar_wait(&empty[s], par ^ 1);
         mbar_arrive_expect_tx(&pk_full[s], kPackedBytes);
         for (int i = 0; i < 8; ++i)
-          bulk_g2s(pk_st + s * kPackedBytes + i * 512, p.qw + ((size_t)(tile0 + i) * p.KB + kb) * 512, 512, &pk_full[s]);
+          bulk_g2s(pk_st + s * kPackedBytes + i * S::kTileBytes, p.qw + ((size_t)(tile0 + i) * p.KB + kb) * S::kTileBytes,
+                   S::kTileBytes, &pk_full[s]);
       }
     }
   } else if (warp == kConsumerWarps + 1 || warp == kConsumerWarps + 2) {
     // ---------------- activation loaders: x block -> B stage in fragment k order ----------------
-    // logical chunk c = 2j + h, word t  <-  physical word 4h + j + 8t  =  component j of input uint4 h + 2t
     const int lt = tid - (kConsumerWarps + 1) * 32;  // 0..63
     for (int kb = 0; kb < p.KB; ++kb) {
       const int s = kb % kStages;
       const uint32_t par = (kb / kStages) & 1;
       mbar_wait(&empty[s], par ^ 1);
       uint8_t* dst = b_st + s * kBBytes;
+      // thread (t, h): token t, half h of the stage's k range
       for (int i = lt; i < p.T_pad * 2; i += 64) {
         const int t = i >> 1, h = i & 1;
-        uint4 v[4];
+        if constexpr (C == Codec::W4) {
+          // logical chunk c = 2j + h, word t  <-  physical word 4h + j + 8t  =  component j of input uint4 h + 2t
+          uint4 v[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          v[u] = make_uint4(0, 0, 0, 0);
-          if (t < p.T) {
-            const int src = kRouted ? rows[t] / src_div : t;
-            v[u] = *reinterpret_cast<const uint4*>(p.x + (size_t)src * p.K + (size_t)kb * BK + (h + 2 * u) * 8);
+          for (int u = 0; u < 4; ++u) {
+            v[u] = make_uint4(0, 0, 0, 0);
+            if (t < p.T) {
+              const int src = kRouted ? rows[t] / src_div : t;
+              v[u] = *reinterpret_cast<const uint4*>(p.x + (size_t)src * p.K + (size_t)kb * BK + (h + 2 * u) * 8);
+            }
           }
+          *reinterpret_cast<uint4*>(dst + sw128_offset(t, 0 + h)) = make_uint4(v[0].x, v[1].x, v[2].x, v[3].x);
+          *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 + h)) = make_uint4(v[0].y, v[1].y, v[2].y, v[3].y);
+          *reinterpret_cast<uint4*>(dst + sw128_offset(t, 4 + h)) = make_uint4(v[0].z, v[1].z, v[2].z, v[3].z);
+          *reinterpret_cast<uint4*>(dst + sw128_offset(t, 6 + h)) = make_uint4(v[0].w, v[1].w, v[2].w, v[3].w);
+        } else if constexpr (C == Codec::F16) {
+          // 16-k blocks 2h, 2h+1; logical chunk (j, hh) of block j, word t  <-  physical word 2t + hh of the block
+          const __half* src = p.x + (size_t)t * p.K + (size_t)kb * S::kK;
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int j = 2 * h + jj;
+            uint4 lo = make_uint4(0, 0, 0, 0), hi = lo;
+            if (t < p.T) {
+              lo = *reinterpret_cast<const uint4*>(src + j * 16);
+              hi = *reinterpret_cast<const uint4*>(src + j * 16 + 8);
+            }
+            *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 * j)) = make_uint4(lo.x, lo.z, hi.x, hi.z);
+            *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 * j + 1)) = make_uint4(lo.y, lo.w, hi.y, hi.w);
+          }
+        } else {
+          // physical words 20h .. 20h+19 of the 40 (lane groups t' = 2h, 2h+1): word 10t' + 5hh + j of the block is word t'
+          // of logical chunk (j, hh), so this thread fills bytes 8h .. 8h+7 of every chunk.  Zero at k >= K (K % 16 == 0:
+          // a uint4 of 8 k lies wholly on one side of K), so nothing past column K of the row is read.
+          const __half* src = p.x + (size_t)t * p.K + (size_t)kb * S::kK;
+          uint4 v[5];
+#pragma unroll
+          for (int u = 0; u < 5; ++u) {
+            v[u] = make_uint4(0, 0, 0, 0);
+            if (t < p.T && kb * S::kK + 40 * h + 8 * u < p.K) v[u] = *reinterpret_cast<const uint4*>(src + 40 * h + 8 * u);
+          }
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(v);
+#pragma unroll
+          for (int j = 0; j < 5; ++j)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+              *reinterpret_cast<uint2*>(dst + w3_offset(t, j, hh) + 8 * h) = make_uint2(w[5 * hh + j], w[10 + 5 * hh + j]);
         }
-        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 0 + h)) = make_uint4(v[0].x, v[1].x, v[2].x, v[3].x);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 2 + h)) = make_uint4(v[0].y, v[1].y, v[2].y, v[3].y);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 4 + h)) = make_uint4(v[0].z, v[1].z, v[2].z, v[3].z);
-        *reinterpret_cast<uint4*>(dst + sw128_offset(t, 6 + h)) = make_uint4(v[0].w, v[1].w, v[2].w, v[3].w);
       }
       fence_async_smem();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
       mbar_arrive(&b_full[s]);
@@ -236,7 +339,17 @@ __device__ __forceinline__ void gemm_w4_cta(const Params& p, uint8_t* smem_raw, 
 template <int NC>
 __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w4_kernel(const __grid_constant__ Params p) {
   extern __shared__ uint8_t smem_raw[];
-  gemm_w4_cta<NC, false>(p, smem_raw, nullptr, 1);
+  gemm_cta<Codec::W4, NC, false>(p, smem_raw, nullptr, 1);
+}
+template <int NC>
+__global__ void __launch_bounds__(kThreads, 1) prefill_gemm_w3_kernel(const __grid_constant__ Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  gemm_cta<Codec::W3, NC, false>(p, smem_raw, nullptr, 1);
+}
+template <int NC>
+__global__ void __launch_bounds__(kThreads, 1) prefill_gemm_f16_kernel(const __grid_constant__ Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  gemm_cta<Codec::F16, NC, false>(p, smem_raw, nullptr, 1);
 }
 
 // ---- grouped MoE GEMM: the same CTA over the slots routed to one expert -------------------------------------------------
@@ -289,7 +402,7 @@ __global__ void __launch_bounds__(kThreads, 1) prefill_moe_gemm_w4_kernel(const 
 #define B200_NC(NC)                                          \
   case NC:                                                   \
     p.T_pad = NC * kNChunk;                                  \
-    gemm_w4_cta<NC, true>(p, smem_raw, rows, mp.src_div);    \
+    gemm_cta<Codec::W4, NC, true>(p, smem_raw, rows, mp.src_div); \
     break;
     B200_NC(1) B200_NC(2) B200_NC(3) B200_NC(4) B200_NC(5) B200_NC(6) B200_NC(7) B200_NC(8)
 #undef B200_NC
@@ -380,24 +493,30 @@ __global__ void silu_mul_kernel(const __half* gu, __half* act, int F) {
 
 using namespace b200;
 
-extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, void* out, int T, b200_stream_t stream) {
-  using namespace b200::prefill;
-  if (!lin || !x || !out || T < 1) return B200_E_INVAL;
-  if (lin->bits != 4 || (lin->group_size > 0 && lin->group_size < lin->K) || (lin->N % BM) || (lin->K % BK) || !lin->qweight ||
-      !lin->scales) {
-    set_error("prefill_gemm_w4: per-channel W4 linear with N % 128 == 0 and K % 64 == 0 required");
-    return B200_E_UNSUPPORTED;
-  }
-  static void (*const kernels[kMaxT / kNChunk])(Params) = {
-      prefill_gemm_w4_kernel<1>, prefill_gemm_w4_kernel<2>, prefill_gemm_w4_kernel<3>, prefill_gemm_w4_kernel<4>,
-      prefill_gemm_w4_kernel<5>, prefill_gemm_w4_kernel<6>, prefill_gemm_w4_kernel<7>, prefill_gemm_w4_kernel<8>};
+namespace b200 {
+namespace prefill {
+
+using GemmKernel = void (*)(Params);
+template <Codec C, int NC>
+constexpr GemmKernel gemm_kernel() {
+  if constexpr (C == Codec::W4) return prefill_gemm_w4_kernel<NC>;
+  else if constexpr (C == Codec::W3) return prefill_gemm_w3_kernel<NC>;
+  else return prefill_gemm_f16_kernel<NC>;
+}
+
+template <Codec C>
+int launch_gemm(const b200_linear_t* lin, const void* x, void* out, int T, cudaStream_t stream) {
+  using S = Stage<C>;
+  static const GemmKernel kernels[kMaxT / kNChunk] = {gemm_kernel<C, 1>(), gemm_kernel<C, 2>(), gemm_kernel<C, 3>(),
+                                                      gemm_kernel<C, 4>(), gemm_kernel<C, 5>(), gemm_kernel<C, 6>(),
+                                                      gemm_kernel<C, 7>(), gemm_kernel<C, 8>()};
   static bool configured[16] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   dev &= 15;
   if (!configured[dev]) {
     for (auto k : kernels) {
-      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::kSmemBytes);
       if (e != cudaSuccess) {
         (void)cudaGetLastError();
         set_error(std::string("prefill_gemm_w4: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
@@ -412,10 +531,10 @@ extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, voi
     p.sz = static_cast<const __half2*>(lin->scales);
     p.x = static_cast<const __half*>(x) + (size_t)t0 * lin->K;
     p.out = static_cast<__half*>(out) + (size_t)t0 * lin->N;
-    p.N = lin->N, p.K = lin->K, p.KB = lin->K / BK, p.T = std::min(kMaxT, T - t0);
+    p.N = lin->N, p.K = lin->K, p.KB = (lin->K + S::kK - 1) / S::kK, p.T = std::min(kMaxT, T - t0);
     const int nc = (p.T + kNChunk - 1) / kNChunk;
     p.T_pad = nc * kNChunk;
-    kernels[nc - 1]<<<lin->N / BM, kThreads, kSmemBytes, static_cast<cudaStream_t>(stream)>>>(p);
+    kernels[nc - 1]<<<lin->N / BM, kThreads, S::kSmemBytes, stream>>>(p);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -423,6 +542,26 @@ extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, voi
     return (int)e;
   }
   return 0;
+}
+
+}  // namespace prefill
+}  // namespace b200
+
+extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, void* out, int T, b200_stream_t stream) {
+  using namespace b200::prefill;
+  if (!lin || !x || !out || T < 1) return B200_E_INVAL;
+  const int bits = lin->bits;
+  const int k_quantum = bits == 3 ? 16 : BK;  // W3: the loaders zero the activations of the padded tail of the last 80-k block
+  if ((bits != 4 && bits != 3 && bits != 16) || (lin->group_size > 0 && lin->group_size < lin->K) || (lin->N % BM) ||
+      (lin->K % k_quantum) || !lin->qweight || (bits != 16 && !lin->scales)) {
+    set_error("prefill_gemm_w4: per-channel W4 / W3 or fp16 linear with N % 128 == 0 and K % 64 == 0 (W3: K % 16 == 0) "
+              "required");
+    return B200_E_UNSUPPORTED;
+  }
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (bits == 4) return launch_gemm<Codec::W4>(lin, x, out, T, st);
+  if (bits == 3) return launch_gemm<Codec::W3>(lin, x, out, T, st);
+  return launch_gemm<Codec::F16>(lin, x, out, T, st);
 }
 
 extern "C" int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_first, int e_count, const int32_t* slot_expert,
@@ -461,7 +600,8 @@ extern "C" int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_firs
   cudaGetDevice(&dev);
   dev &= 15;
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(prefill_moe_gemm_w4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(prefill_moe_gemm_w4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)Stage<Codec::W4>::kSmemBytes);
     if (e != cudaSuccess) {
       (void)cudaGetLastError();
       set_error(std::string("prefill_moe_gemm_w4: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
@@ -470,7 +610,7 @@ extern "C" int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_firs
     configured[dev] = true;
   }
   const dim3 grid(mp.N / BM, e_count, (n_slots + kMaxT - 1) / kMaxT);
-  prefill_moe_gemm_w4_kernel<<<grid, kThreads, kSmemBytes, static_cast<cudaStream_t>(stream)>>>(mp);
+  prefill_moe_gemm_w4_kernel<<<grid, kThreads, Stage<Codec::W4>::kSmemBytes, static_cast<cudaStream_t>(stream)>>>(mp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error(std::string("prefill_moe_gemm_w4: launch: ") + cudaGetErrorString(e));

@@ -650,16 +650,21 @@ class DecodeEngine:
 
     # ------------------------------------------------------------------ prefill on the tensor cores ----
     T_PREFILL = 256  # tokens per wgmma GEMM launch (a CTA holds 128 rows x 256 tokens of fp32 accumulators)
+    # shortest prompt the tensor-core path takes, per codec (default: longer than one 32-token GEMV chunk).  W3 prompts of
+    # 33 and 40 tokens ran as fast through the GEMV chunks, 48 tokens 11 % faster on the tensor cores (DESIGN.md 4.6)
+    TC_MIN_PROMPT = {3: 48}
 
     def prefill_tc_supported(self):
-        """Per-channel W4 dense LLaMA or Mixtral whose linears (experts included) tile by 128 output rows: prompts go through
-        b200_prefill_gemm_w4 and, for the experts, b200_prefill_moe_gemm_w4."""
+        """Dense LLaMA with per-channel W4 / W3 or fp16 linears, or per-channel W4 Mixtral, whose linears (experts included)
+        tile by 128 output rows: prompts go through b200_prefill_gemm_w4 and, for the experts, b200_prefill_moe_gemm_w4."""
         c = self.cfg
-        if not self.use_prefill_tc or c.kind not in ("llama", "mixtral") or c.bits != 4 or c.group_size or self.shard_only:
+        codecs = (4, 3, 16) if c.kind == "llama" else (4,)
+        if (not self.use_prefill_tc or c.kind not in ("llama", "mixtral") or c.bits not in codecs or c.group_size
+                or self.shard_only):
             return False
         lw = self.layers[0]
         lins = (lw.wqkv, lw.wo, lw.w13, lw.w2) if c.kind == "llama" else (lw.wqkv, lw.wo, *lw.e_w13, *lw.e_w2)
-        return all(pl.N % 128 == 0 and pl.K % 64 == 0 for pl in lins)
+        return all(pl.N % 128 == 0 and pl.K % (16 if pl.bits == 3 else 64) == 0 for pl in lins)
 
     def _prefill_bufs(self):
         if self._pf is None:
@@ -847,7 +852,8 @@ class DecodeEngine:
             return self.decode_step(tokens[:, 0].contiguous(), start_pos)
         # prefill: chunks of <= t_max tokens walk the layer stack in order (each chunk only needs the
         # K/V of earlier chunks); sequences are processed in groups when bsz alone exceeds t_max
-        if (seqlen > T_MAX or self.force_tc) and self.prefill_tc_supported():
+        tc_min = self.TC_MIN_PROMPT.get(self.cfg.bits, T_MAX + 1)
+        if (seqlen >= tc_min or self.force_tc) and self.prefill_tc_supported():
             # tensor-core prefill: one sequence at a time, chunks of <= 256 positions
             outs = []
             for b0 in range(bsz):

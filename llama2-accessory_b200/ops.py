@@ -123,7 +123,8 @@ def _anchor(t, name):
 
 
 def prefill_gemm_w4(lin: PackedLinear, x, out, T):
-    """out[T, N] = x[T, K] . w_hat^T on the tensor cores (wgmma) (per-channel W4, N % 128 == 0)."""
+    """out[T, N] = x[T, K] . w_hat^T on the tensor cores (wgmma): per-channel W4 or W3, or fp16 weights (w_hat = w);
+    N % 128 == 0, K % 64 == 0 (W3: K % 16 == 0)."""
     global launch_count
     on = _anchor(x, "x")
     _dev(x, "x", torch.float16, T * lin.K, on)
