@@ -1,10 +1,12 @@
 """Shared numerics helpers of the kernel tests: fp16 rounding sides, the fp32 rstd window of the RMSNorm prologues,
-NaN-sentinel buffers, set-and-restore of a b200_tune knob, and the line-by-line model of moe_route_kernel's routing.
+NaN-sentinel buffers, set-and-restore of a b200_tune knob, the line-by-line model of moe_route_kernel's routing, and the
+split schedules and step-by-step arithmetic model of the decode attention kernel.
 
 Test infrastructure only (see oracle/__init__.py).  Every function here is plain torch / numpy; the CUDA library is only
 touched by `tuned`, and only when it is entered.
 """
 import contextlib
+import math
 import os
 
 import numpy as np
@@ -14,7 +16,8 @@ SENT = 0x7E5A      # NaN bit pattern: a sentinel no kernel writes
 RSTD_ULPS = 32     # the kernels' fp32 rstd lies within this many fp32 ulps of rstd64 (test_decode_path_gpu.py derives it)
 
 # what a b200_tune knob is when neither a b200_tune call nor the environment sets it (csrc: tune_get defaults)
-TUNE_DEFAULTS = {"B200_PF_EARLY": 0, "B200_SELF_PF_KB": 0, "B200_STREAM_EF": 1, "B200_QKV_RING_KB": 0, "B200_GEMV1": 1}
+TUNE_DEFAULTS = {"B200_PF_EARLY": 0, "B200_SELF_PF_KB": 0, "B200_STREAM_EF": 1, "B200_QKV_RING_KB": 0, "B200_GEMV1": 1,
+                 "B200_ATTN_EVEN": 0, "B200_ATTN_MAX_SPLIT": 16, "B200_KV_EF": 1}
 
 
 def nan16(*shape, device="cuda"):
@@ -96,3 +99,95 @@ def kernel_route(logits16, k):
     s16 = s.astype(np.float16).astype(np.float32)
     w = (val / s16[:, None]).astype(np.float32).astype(np.float16)
     return torch.from_numpy(idx), torch.from_numpy(w)
+
+
+# ------------------------------------------------------------------------------------- decode attention model --------
+ATTN_TILE, ATTN_WARPS = 32, 4      # kv positions per tile, consumer warps per CTA (csrc/attn.cu kTile, kAttnWarps)
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def attn_choose_split(T, Hkv, max_kv_len, sms, cap=16):
+    """b200_attn_choose_split: enough splits for two CTAs per SM, at most one per 128 keys, capped at `cap`
+    (B200_ATTN_MAX_SPLIT) only while the capped grid still gives every SM a CTA; then rounded to whole 32-key chunks."""
+    if T <= 0 or Hkv <= 0 or max_kv_len <= 0:
+        return 1
+    want = 2 * sms // (T * Hkv)
+    want = max(1, min(want, _cdiv(max_kv_len, ATTN_WARPS * ATTN_TILE)))
+    if want > cap and T * Hkv * cap >= sms:
+        want = max(cap, 1)
+    chunk = _cdiv(_cdiv(max_kv_len, want), ATTN_TILE) * ATTN_TILE
+    return _cdiv(max_kv_len, chunk)
+
+
+def attn_host_split(max_kv_len, n_split):
+    """b200_attn_decode: a requested split count -> (split count launched, chunk).  The chunk is a whole number of tiles,
+    so a request above max_kv_len / 32 launches one split per tile."""
+    chunk = _cdiv(_cdiv(max_kv_len, n_split), ATTN_TILE) * ATTN_TILE
+    return _cdiv(max_kv_len, chunk), chunk
+
+
+def attn_split_ranges(kv_len, n_split, chunk, even):
+    """[(s_begin, s_end)] of every split of one token whose keys are 0 .. kv_len - 1 (attn_decode_kernel); s_end <= s_begin
+    is an empty split.
+      even = 0: equal chunks rounded up to whole tiles, sized for the ACTUAL kv_len but never above the launch's chunk;
+      even = 1 (B200_ATTN_EVEN): the n_t tiles holding keys dealt out, split i taking tiles [n_t i / n, n_t (i + 1) / n)."""
+    out = []
+    for sp in range(n_split):
+        if even:
+            n_t = _cdiv(kv_len, ATTN_TILE)
+            b, e = n_t * sp // n_split * ATTN_TILE, min(kv_len, n_t * (sp + 1) // n_split * ATTN_TILE)
+        else:
+            c = min(chunk, _cdiv(_cdiv(kv_len, n_split), ATTN_TILE) * ATTN_TILE)
+            b = sp * c
+            e = min(kv_len, b + c)
+        out.append((b, max(b, e)))
+    return out
+
+
+def attn_kernel_model(q, k, v, n_split, even=False, max_kv_len=None):
+    """q fp16 [128], k / v fp16 [n, 128] (positions 0 .. pos) -> fp16 [128], following attn.cu step by step in torch fp32.
+
+        scores   fp16 q . fp16 k accumulated in fp32, times scale_log2 = fp32(fp32(1/sqrt(128)) * fp32(log2 e))
+        splits   the grid b200_attn_decode launches for (max_kv_len, n_split), cut by attn_split_ranges
+        warps    inside a split, tile i belongs to consumer warp i % 4; a warp folds ITS tiles in order with the online rule
+                 m' = max(m, max_tile), corr = 2^(m - m'), l = l corr + sum(fp16(p)), O = O corr + fp16(p) V, p = 2^(s - m')
+        merge    4 warps, then the splits in split order: M = max m, f = 2^(m - M) (0 for an empty part), L = sum l f,
+                 o = sum O f; out = fp16(o / L)
+    The kernel's HMMA accumulates in another order and its exp2f is not torch's exp2: the model and the kernel agree to a
+    few fp16 steps, not bit for bit."""
+    n = k.shape[0]
+    ns, chunk = attn_host_split(max_kv_len or n, n_split)
+    scale_log2 = torch.tensor(1.0 / math.sqrt(128.0), dtype=torch.float32) * torch.tensor(1.4426950408889634,
+                                                                                          dtype=torch.float32)
+    s_all = (k.float() @ q.float()) * scale_log2                                         # fp32 accumulation of exact products
+    ninf = torch.tensor(-math.inf)
+
+    def fold(parts):                                                                     # [(m, l, o)] in order -> (M, L, o)
+        M = torch.stack([m for m, _, _ in parts]).max()
+        L, o = torch.tensor(0.0), torch.zeros(128)
+        for m, l, oo in parts:
+            f = torch.tensor(0.0) if m == -math.inf else torch.exp2(m - M)
+            L, o = L + l * f, o + oo * f
+        return M, L, o
+    splits = []
+    for s_begin, s_end in attn_split_ranges(n, ns, chunk, even):
+        n_tiles = _cdiv(s_end - s_begin, ATTN_TILE)
+        warps = []
+        for w in range(ATTN_WARPS):
+            m, l, o = ninf, torch.tensor(0.0), torch.zeros(128)
+            for i in range(w, n_tiles, ATTN_WARPS):
+                a, b = s_begin + i * ATTN_TILE, min(s_end, s_begin + (i + 1) * ATTN_TILE)
+                s = s_all[a:b]
+                m_new = torch.maximum(m, s.max())
+                corr = torch.exp2(m - m_new)
+                p16 = torch.exp2(s - m_new).half()                                       # P rounded for the second MMA
+                l = l * corr + p16.float().sum()
+                o = o * corr + p16.float() @ v[a:b].float()
+                m = m_new
+            warps.append((m, l, o))
+        splits.append(fold(warps))
+    _, L, o = fold(splits)
+    return (o / L).half()

@@ -9,51 +9,36 @@ against an exact softmax attention and against the reference's own fp16 SDPA cal
                 result stays a convex combination of V rows (no normalisation bias)
     merge       4 warps, then the splits in split order: M = max m, f = 2^(m - M), L = sum l f, o = sum O f; out = fp16(o / L)
 
-No GPU: this pins the numerics MODEL (DESIGN.md section 2), the kernel itself is compared with an fp32 reference by
-tests/test_kernels_gpu.py::test_attn_decode.
+No GPU: this pins the numerics MODEL (DESIGN.md section 2, oracle.numerics.attn_kernel_model); the kernel itself is
+compared with float64 and with this model by tests/test_attn_decode_gpu.py.
 """
 import math
 
 import pytest
 import torch
 
-TILE, WARPS = 32, 4
+from oracle.numerics import ATTN_TILE as TILE
+from oracle.numerics import attn_host_split, attn_kernel_model as kernel_model, attn_split_ranges
 
 
-def kernel_model(q, k, v, n_split):
-    """q fp16 [128], k / v fp16 [n, 128] (positions 0..pos) -> fp16 [128], following attn.cu step by step in torch fp32."""
-    n = k.shape[0]
-    scale_log2 = (1.0 / math.sqrt(128.0)) * 1.4426950408889634
-    chunk = -(-n // n_split)
-    chunk = -(-chunk // TILE) * TILE
-    n_split = -(-n // chunk)
-    s_all = (k.float() @ q.float()) * torch.tensor(scale_log2, dtype=torch.float32)      # fp32 accumulation of exact products
-    parts = []                                                                           # per split: (M, L, o[128])
-    for sp in range(n_split):
-        s_begin, s_end = sp * chunk, min(n, (sp + 1) * chunk)
-        n_tiles = -(-(s_end - s_begin) // TILE)
-        warps = []
-        for w in range(WARPS):
-            m, l, o = torch.tensor(-math.inf), torch.tensor(0.0), torch.zeros(128)
-            for i in range(w, n_tiles, WARPS):
-                a, b = s_begin + i * TILE, min(s_end, s_begin + (i + 1) * TILE)
-                s = s_all[a:b]
-                m_new = torch.maximum(m, s.max())
-                corr = torch.exp2(m - m_new)
-                p16 = torch.exp2(s - m_new).half()                                       # P rounded for the second MMA
-                l = l * corr + p16.float().sum()
-                o = o * corr + p16.float() @ v[a:b].float()
-                m = m_new
-            warps.append((m, l, o))
-        M = torch.stack([m for m, _, _ in warps]).max()
-        f = [torch.tensor(0.0) if m == -math.inf else torch.exp2(m - M) for m, _, _ in warps]
-        parts.append((M, sum(l * fi for (_, l, _), fi in zip(warps, f)), sum(o * fi for (_, _, o), fi in zip(warps, f))))
-    M = torch.stack([m for m, _, _ in parts]).max()
-    L, o = torch.tensor(0.0), torch.zeros(128)
-    for m, l, oo in parts:                                                               # split order
-        f = torch.exp2(m - M)
-        L, o = L + l * f, o + oo * f
-    return (o / L).half()
+@pytest.mark.parametrize("even", [0, 1])
+@pytest.mark.parametrize("max_kv_len", [1, 31, 32, 33, 200, 2048, 2400, 4096, 32768])
+def test_both_split_schedules_cut_every_context_into_whole_tiles_once(max_kv_len, even):
+    """Every kv length up to the launch's max_kv_len, every requested split count: the non-empty splits are consecutive,
+    cover [0, kv_len) once, begin on a tile, and none exceeds the launch's chunk; the even schedule's tile counts differ by
+    at most one."""
+    for req in sorted({1, 2, 3, 7, 16, 17, 33, max(1, max_kv_len // 32), max_kv_len // 32 + 5}):
+        ns, chunk = attn_host_split(max_kv_len, req)
+        assert ns <= req and chunk % TILE == 0 and (ns - 1) * chunk < max_kv_len <= ns * chunk
+        for kv_len in sorted({1, 2, 31, 32, 33, max_kv_len // 2 + 1, max_kv_len - 1, max_kv_len} - {0}):
+            if kv_len > max_kv_len:
+                continue
+            r = [(b, e) for b, e in attn_split_ranges(kv_len, ns, chunk, even) if e > b]
+            assert r[0][0] == 0 and r[-1][1] == kv_len and all(r[i][1] == r[i + 1][0] for i in range(len(r) - 1))
+            assert all(b % TILE == 0 and e - b <= chunk for b, e in r), (req, kv_len, r)
+            if even:
+                nt = [-(-(e - b) // TILE) for b, e in attn_split_ranges(kv_len, ns, chunk, even)]
+                assert max(nt) - min(nt) <= 1, (req, kv_len, nt)
 
 
 def exact(q, k, v):
@@ -72,6 +57,20 @@ def test_kernel_arithmetic_model_is_within_half_precision_of_exact_attention(n, 
     # output rounding (half an fp16 ulp of the value) + the fp16 rounding of P (relative 2^-11 per weight, averaged out)
     tol = 2.0 ** -11 * ref.abs().clamp(min=2.0 ** -6) + 2.0 ** -11 * float(v.float().abs().max())
     assert ((got - ref).abs() <= tol).all(), float((got - ref).abs().max())
+
+
+@pytest.mark.parametrize("n,n_split,max_kv_len", [(33, 16, 4096), (200, 3, 200), (2048, 16, 2048), (2049, 7, 4096)])
+def test_even_schedule_model_is_within_half_precision_of_exact_attention(n, n_split, max_kv_len):
+    """B200_ATTN_EVEN = 1 and a grid sized for a longer context than the keys present (the captured-graph case)."""
+    g = torch.Generator().manual_seed(n * 17 + n_split)
+    q = torch.randn(128, generator=g).half()
+    k = torch.randn(n, 128, generator=g).half()
+    v = (torch.randn(n, 128, generator=g) * 0.5).half()
+    ref = exact(q, k, v)
+    tol = 2.0 ** -11 * ref.abs().clamp(min=2.0 ** -6) + 2.0 ** -11 * float(v.float().abs().max())
+    for even in (False, True):
+        got = kernel_model(q, k, v, n_split, even=even, max_kv_len=max_kv_len).double()
+        assert ((got - ref).abs() <= tol).all(), (even, float((got - ref).abs().max()))
 
 
 def test_split_count_moves_the_result_by_at_most_one_output_rounding_step():

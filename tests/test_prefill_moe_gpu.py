@@ -271,7 +271,9 @@ def _schedule(model, toks, p0, p1, ndec):
 def test_mixtral_continuation_prompt_matches_port(p0, p1):
     """A second prompt at start_pos = p0 > 0, then decode; the tensor-core path's logits and KV cache meet the port rule.
     The GEMV-chunk path (unchanged here) is run and recorded, not asserted: at (40, 300) it measured e32 = 2.2e-2 against
-    a floor of 2.6e-3 on an H100, while the tensor-core path met the rule; the cause is not diagnosed."""
+    a floor of 2.6e-3 on an H100, while the tensor-core path met the rule; the cause is not diagnosed.  Attention is
+    cleared there: every attention launch of that schedule (16 tokens / 8 per sequence, and the last 8 / 4) meets the
+    float64 bound and the exact probes of test_attn_decode_gpu.py::test_engine_launch_shapes[tiny_mixtral_40_300]."""
     args, sd, sd_ref, recs = _tiny_mixtral()
     ndec, P = 3, p0 + p1
     toks = weights.synthetic_tokens(2, P + ndec, args["vocab_size"], seed=11)
