@@ -87,6 +87,12 @@ class PortModel:
         self.freqs_cis = precompute_freqs_cis(self.hd, self.max_seq_len * 2, theta, a.get("rope_scaling")).to(self.device)
         assert self.H % tp == 0 and self.Hkv % tp == 0
         self.k_cache = self.v_cache = None
+        # diagnosis aids, both off by default: `record` (a list) receives one dict per forward_inference call with the
+        # residual stream after every block and the experts each token was routed to; `force_routes` maps
+        # (start_pos, layer) -> int64 [B * S, k] expert ids that MoE uses instead of its own top-k (in that slot order)
+        self.record = None
+        self.force_routes = None
+        self._start_pos = 0
         if kind == "mixtral":
             self.E = a["moe"]["num_experts"]
             self.topk = a["moe"]["num_experts_per_tok"]
@@ -153,6 +159,15 @@ class PortModel:
         x = x.view(-1, shp[-1])
         scores = F.linear(x, self._w(p + "gate.weight")).softmax(dim=-1).to(x)
         ew, ei = torch.topk(scores, self.topk, dim=-1)
+        if self.record is not None:  # the model's own top-k, and its scores
+            self.record[-1]["own"].append(ei.view(*shp[:-1], self.topk).cpu().clone())
+            self.record[-1]["scores"].append(scores.view(*shp[:-1], -1).float().cpu().clone())
+        forced = (self.force_routes or {}).get((self._start_pos, i))
+        if forced is not None:
+            ei = forced.to(self.device).long().view(-1, self.topk)
+            ew = scores.gather(-1, ei)
+        if self.record is not None:  # the experts used
+            self.record[-1]["routes"].append(ei.view(*shp[:-1], self.topk).cpu().clone())
         flat = ei.view(-1)
         ew = ew / ew.sum(dim=-1, keepdim=True)
         xr = x.repeat_interleave(self.topk, dim=0)
@@ -183,8 +198,13 @@ class PortModel:
             self.alloc_cache(B)
         h = F.embedding(tokens, self._w("tok_embeddings.weight"))
         fc = self.freqs_cis[start_pos:start_pos + S]
+        self._start_pos = start_pos
+        if self.record is not None:
+            self.record.append(dict(start_pos=start_pos, h=[], routes=[], own=[], scores=[]))
         for i in range(self.L):
             h = self.block(i, h, start_pos, fc, causal=(S != 1))
+            if self.record is not None:
+                self.record[-1]["h"].append(h.cpu().clone())
         hn = rmsnorm(h, self._w("norm.weight"), self.eps)
         logits = F.linear(hn[:, -1, :], self._w("output.weight")).float()
         return (logits, h) if return_hidden else logits

@@ -2,10 +2,16 @@
 NaN-sentinel buffers, set-and-restore of a b200_tune knob, the line-by-line model of moe_route_kernel's routing, and the
 split schedules and step-by-step arithmetic model of the decode attention kernel.
 
+Also the float64 checkers that more than one GPU module applies (their bounds are derived in the docstrings of
+tests/test_gemv_batched_moe_gpu.py, sections A and B, and tests/test_attn_decode_gpu.py, section A): the GEMV bound,
+the RoPE of the QKV epilogue, the SiLU-product range, the router's logit window and routing check, and the float64
+reference and bound of decode attention.
+
 Test infrastructure only (see oracle/__init__.py).  Every function here is plain torch / numpy; the CUDA library is only
 touched by `tuned`, and only when it is entered.
 """
 import contextlib
+import itertools
 import math
 import os
 
@@ -14,6 +20,10 @@ import torch
 
 SENT = 0x7E5A      # NaN bit pattern: a sentinel no kernel writes
 RSTD_ULPS = 32     # the kernels' fp32 rstd lies within this many fp32 ulps of rstd64 (test_decode_path_gpu.py derives it)
+C_ACC = 2.0 ** -18       # fp32 accumulation constant of the fp16 HMMA kernels, relative to |x| . |w|^T (test_prefill_gpu.py)
+SILU_REL = 2.0 ** -20    # fp32 a / (1 + expf(-a)): <= 3.5 u << 16 u (test_decode_path_gpu.py)
+SILU_ARGMIN = -1.2784645427610737  # silu has its only minimum there
+MAX_AMB = 12             # router: at most 2^12 rounding choices of ambiguous logits per token
 
 # what a b200_tune knob is when neither a b200_tune call nor the environment sets it (csrc: tune_get defaults)
 TUNE_DEFAULTS = {"B200_PF_EARLY": 0, "B200_SELF_PF_KB": 0, "B200_STREAM_EF": 1, "B200_QKV_RING_KB": 0, "B200_GEMV1": 1,
@@ -191,3 +201,186 @@ def attn_kernel_model(q, k, v, n_split, even=False, max_kv_len=None):
         splits.append(fold(warps))
     _, L, o = fold(splits)
     return (o / L).half()
+
+
+# ------------------------------------------------------------------------------------------- GEMV bound ------------
+def _bits16(t):
+    return t.contiguous().view(torch.int16)
+
+
+def gemv_tol(ref, M):
+    """The element-wise bound of the multi-token GEMV against float64 ref, M = A . |x| (test_gemv_batched_moe_gpu.py, A)."""
+    return ref.abs() * 2.0 ** -11 + C_ACC * M * (1 + 2.0 ** -10) + 2.0 ** -25
+
+
+def gemv_check(out, ref, M, label):
+    """out [T, N] against float64 ref with the GEMV bound -> (worst err / tol, implied C, exact fraction)."""
+    o = out.double()
+    assert torch.isfinite(o).all(), label
+    err = (o - ref).abs()
+    tol = gemv_tol(ref, M)
+    ratio = float((err / tol).max())
+    c_seen = float(((err - ref.abs() * 2.0 ** -11).clamp_min(0) / M.clamp_min(1e-30)).max())
+    exact = float((_bits16(out) == _bits16(ref.half())).double().mean())
+    assert ratio <= 1.0, (label, ratio)
+    return ratio, c_seen, exact
+
+
+def rope_rotate(y16, cs):
+    """fp32 RoPE of the QKV epilogue as separate multiplies and adds: y16 [rows] fp16 of whole heads, cs [rows / 2, 2]."""
+    p = y16.float().reshape(-1, 2)
+    e, o = p[:, 0], p[:, 1]
+    c, s = cs[:, 0], cs[:, 1]
+    return torch.stack([e * c - o * s, e * s + o * c], dim=-1).reshape(-1).half()
+
+
+def qkv_from_y(y, rope, pos, n_q_rows, n_kv_rows):
+    """The QKV epilogue's outputs as a function of the F16 launch's y [T, n_q + 2 n_kv] on the same inputs -> (q [T, n_q],
+    k [T, n_kv], v [T, n_kv]) fp16: q and k rotated by rope[pos[t]], v = y."""
+    rows = []
+    for t in range(y.shape[0]):
+        cs = rope[int(pos[t])].repeat((n_q_rows + n_kv_rows) // 128, 1)
+        rows.append(rope_rotate(y[t, :n_q_rows + n_kv_rows], cs))
+    r = torch.stack(rows)
+    return r[:, :n_q_rows], r[:, n_q_rows:], y[:, n_q_rows + n_kv_rows:]
+
+
+def silu_mul_range(ya, ta, yb, tb):
+    """[lo, hi] of fp16(fp16(silu(a)) * b) over every fp16 a = fp16(y), |y - ya| <= ta (b likewise): fp16 rounding and
+    the product are monotone, silu is monotone on each side of its minimum, and the fp32 silu lies within SILU_REL."""
+    def silu(a):
+        return a / (1 + torch.exp(-a))
+    a_lo, a_hi = (ya - ta).half().double(), (ya + ta).half().double()
+    b_lo, b_hi = (yb - tb).half().double(), (yb + tb).half().double()
+    s1, s2 = silu(a_lo), silu(a_hi)
+    smin = torch.minimum(s1, s2)
+    smin = torch.where((a_lo <= SILU_ARGMIN) & (a_hi >= SILU_ARGMIN), torch.full_like(smin, silu(torch.tensor(SILU_ARGMIN, dtype=torch.float64)).item()), smin)
+    smax = torch.maximum(s1, s2)
+    s_lo = (smin - SILU_REL * smin.abs()).half().double()
+    s_hi = (smax + SILU_REL * smax.abs()).half().double()
+    c = torch.stack([s_lo * b_lo, s_lo * b_hi, s_hi * b_lo, s_hi * b_hi])
+    return c.amin(0).half().double(), c.amax(0).half().double()
+
+
+# -------------------------------------------------------------------------------------------- router check ----------
+def logit_window(xn, gate):
+    """float64 logits and the running-error bound R of moe_route_kernel's lane chains + warp tree
+    (test_gemv_batched_moe_gpu.py, B)."""
+    T, D = xn.shape
+    E = gate.shape[0]
+    p = xn.double()[:, None, :] * gate.double()[None]                       # [T, E, D] exact products
+    # lane l owns uint4 chunks u = l, l + 32, ...: elements 8u .. 8u + 7 in order
+    p = p.reshape(T, E, D // 256, 32, 8).permute(0, 1, 3, 2, 4).reshape(T, E, 32, D // 32)
+    part = p.cumsum(-1)
+    lane = part[..., -1]
+    R = 2.0 ** -24 * (part.abs().sum(-1).sum(-1) + 5 * lane.abs().sum(-1)) * (1 + 2.0 ** -10)
+    L = lane.sum(-1)
+    assert bool((R <= (D / 32 + 5) * 2.0 ** -24 * (xn.double().abs() @ gate.double().abs().T) * 1.01).all())
+    return L, R
+
+
+def route_scores32(logits16):
+    """fp16 [T, E] logits -> the kernel's fp32 softmax scores (experts summed in index order) as float64, unrounded."""
+    lg = logits16.float().cpu().numpy()
+    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
+    den = np.zeros(lg.shape[0], dtype=np.float32)
+    for e in range(lg.shape[1]):
+        den = (den + ex[:, e]).astype(np.float32)
+    return torch.from_numpy((ex / den[:, None]).astype(np.float32)).double()
+
+
+def route_check(xn, gate, sw, se, k, max_amb=MAX_AMB):
+    """moe_route's slot_expert / slot_weight [T, k] against every kernel_route outcome of the logit window of its own
+    xn_out -> (tokens matched bit for bit, tokens in the expf window, tokens with too many ambiguous logits)."""
+    L, R = logit_window(xn, gate)
+    near, alt, dist = fp16_sides(L)
+    amb = (dist <= R).cpu()
+    near, alt = near.cpu(), alt.cpu()
+    se_c, sw_c = se.cpu().long(), _bits16(sw).cpu()
+    matched = window = skipped = 0
+    for t in range(L.shape[0]):
+        ai = torch.nonzero(amb[t]).reshape(-1).tolist()
+        if len(ai) > max_amb:
+            skipped += 1
+            continue
+        combos = torch.tensor(list(itertools.product([0, 1], repeat=len(ai))), dtype=torch.bool).reshape(2 ** len(ai), len(ai))
+        C = near[t].repeat(combos.shape[0], 1)
+        if ai:
+            C[:, ai] = torch.where(combos, alt[t, ai][None].expand_as(combos), near[t, ai][None].expand_as(combos))
+        lg16 = C.half()
+        idx, w = kernel_route(lg16, k)
+        hit = (idx == se_c[t][None]).all(1) & (w.view(torch.int16) == sw_c[t][None]).all(1)
+        if bool(hit.any()):
+            matched += 1
+            continue
+        s = route_scores32(lg16)
+        _, _, sd = fp16_sides(s)
+        assert bool((sd <= 2.0 ** -20 * s.abs()).any()), (t, se_c[t].tolist(), idx[:4].tolist())
+        window += 1
+    return matched, window, skipped
+
+
+# ------------------------------------------------------------------------------------ decode attention bound --------
+ATTN_U = 2.0 ** -24
+ATTN_EXP2_REL = 2.0 ** -22           # exp2f: 2 ulp
+ATTN_C_LOG2 = 1.4426950408889634 / math.sqrt(128.0)
+
+
+def attn_tiles_per_warp(kv_len, n_split, chunk, even):
+    """largest number of tiles one consumer warp of attn_decode_kernel folds for a token."""
+    return max(_cdiv(_cdiv(e - b, ATTN_TILE), ATTN_WARPS) for b, e in attn_split_ranges(kv_len, n_split, chunk, even))
+
+
+class AttnRef:
+    """float64 attention of every (token, head) of a decode-attention launch and the sums its bound is made of
+    (test_attn_decode_gpu.py, A).  q [T, Hq, 128], k / v canonical [B, Hkv, S, 128] fp16, token t of sequence t // tps
+    attends to rows 0 .. pos[t]."""
+
+    def __init__(self, q, k, v, pos, tps):
+        T, Hq, _ = q.shape
+        Hkv = k.shape[1]
+        r = Hq // Hkv
+        dev = q.device
+        z3 = lambda: torch.zeros(T, Hq, 128, dtype=torch.float64, device=dev)  # noqa: E731
+        z2 = lambda: torch.zeros(T, Hq, dtype=torch.float64, device=dev)  # noqa: E731
+        self.out, self.s_eps, self.s_dev, self.s_sub, self.s_absv = z3(), z3(), z3(), z3(), z3()
+        self.sw, self.w_eps, self.n_sub = z2(), z2(), z2()
+        self.pos = [int(p) for p in pos]
+        for t in range(T):
+            b, n = t // tps, self.pos[t] + 1
+            for g in range(Hkv):
+                hs = slice(g * r, (g + 1) * r)
+                qq, kk, vv = q[t, hs].double(), k[b, g, :n].double(), v[b, g, :n].double()
+                tl = (qq @ kk.T) * ATTN_C_LOG2
+                tmax = tl.max(-1, keepdim=True).values
+                w = torch.exp2(tl - tmax)
+                sw = w.sum(-1)
+                o = (w @ vv) / sw[:, None]
+                dlt = C_ACC * ATTN_C_LOG2 * (qq.abs() @ kk.abs().T) + 16 * ATTN_U * torch.maximum(tl.abs(), tmax.abs())
+                eps = torch.exp2(dlt) - 1 + 2.0 ** -11
+                sub = (w < 2.0 ** -13).double()
+                dev_ = (vv[None] - o[:, None]).abs()
+                self.out[t, hs], self.sw[t, hs] = o, sw
+                self.s_eps[t, hs] = torch.einsum("rn,rnd->rd", w * eps, dev_)
+                self.s_dev[t, hs] = torch.einsum("rn,rnd->rd", w, dev_)
+                self.s_sub[t, hs] = torch.einsum("rn,rnd->rd", sub, dev_)
+                self.s_absv[t, hs] = w @ vv.abs()
+                self.w_eps[t, hs], self.n_sub[t, hs] = (w * eps).sum(-1), sub.sum(-1)
+
+    def tol(self, tpw, n_split):
+        """tpw: tiles per warp of every token (list)."""
+        U = ATTN_U
+        tw = torch.tensor(tpw, dtype=torch.float64, device=self.out.device).view(-1, 1)
+        ec = (tw + 3) * ATTN_EXP2_REL
+        den = self.sw - self.w_eps - ec * self.sw - 2.0 ** -25 * self.n_sub
+        assert bool((den > 0).all())
+        p_err = (2 * (self.s_eps + ec[..., None] * self.s_dev) + 2 * 2.0 ** -25 * self.s_sub) / den[..., None]
+        acc = ((C_ACC + (tw[..., None] + n_split + 8) * U) * self.s_absv / self.sw[..., None]
+               + (5 * tw[..., None] + n_split // 32 + 20) * U * self.out.abs())
+        return (p_err + acc) * (1 + 2.0 ** -11) + 2.0 ** -11 * self.out.abs() + 2.0 ** -25
+
+    def ratio(self, out, n_split, chunk, even):
+        """max err / tol of the kernel's out [T, Hq, 128] launched with (n_split, chunk) under schedule `even`."""
+        assert bool(torch.isfinite(out).all()), "non-finite output"
+        tpw = [attn_tiles_per_warp(p + 1, n_split, chunk, even) for p in self.pos]
+        return float(((out.double() - self.out).abs() / self.tol(tpw, n_split)).max())

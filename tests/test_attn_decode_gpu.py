@@ -65,8 +65,6 @@ log2 units, w_i = 2^(t_i - max t) its weight (the largest is 1), out = sum w V /
   torch's exp2 is not exp2f, so no sharp bound between the two follows from the above: the difference is reported in fp16
   ulps, not asserted.
 """
-import math
-
 import pytest
 import torch
 
@@ -76,12 +74,10 @@ import llama2_accessory_b200 as pkg  # noqa: E402
 from llama2_accessory_b200 import _cabi, kvlayout, ops  # noqa: E402
 from oracle.numerics import SENT, attn_choose_split, attn_host_split, attn_kernel_model, attn_split_ranges  # noqa: E402
 from oracle.numerics import nan16, tuned  # noqa: E402
+# the float64 reference and bound of section A live in oracle/numerics.py, shared with test_engine_launch_audit_gpu.py
+from oracle.numerics import AttnRef as _Ref  # noqa: E402
 
 DEV = "cuda"
-U = 2.0 ** -24
-C_ACC = 2.0 ** -18              # fp32 HMMA accumulation, relative to the sum of |products| (see above)
-EXP2_REL = 2.0 ** -22           # exp2f: 2 ulp
-C_LOG2 = 1.4426950408889634 / math.sqrt(128.0)
 PROBE_Q, PROBE_K = 16.0, 32.0   # selection probe: gap 65.3 log2 units
 PAD = 512                       # NaN margin on each side of the output
 S4K = 4096
@@ -138,64 +134,8 @@ def _cdiv(a, b):
     return -(-a // b)
 
 
-def _tpw(kv_len, n_split, chunk, even):
-    """largest number of tiles one consumer warp folds for a token."""
-    return max(_cdiv(_cdiv(e - b, 32), 4) for b, e in attn_split_ranges(kv_len, n_split, chunk, even))
-
-
 def _bits(x):
     return x.contiguous().view(torch.int16)
-
-
-# ---------------------------------------------------------------------------------------- float64 reference --------
-class _Ref:
-    """float64 attention of every (token, head) of a launch and the sums its bound is made of (module docstring, A)."""
-
-    def __init__(self, q, k, v, pos, tps):
-        T, Hq, _ = q.shape
-        Hkv = k.shape[1]
-        r = Hq // Hkv
-        z3 = lambda: torch.zeros(T, Hq, 128, dtype=torch.float64, device=DEV)  # noqa: E731
-        z2 = lambda: torch.zeros(T, Hq, dtype=torch.float64, device=DEV)  # noqa: E731
-        self.out, self.s_eps, self.s_dev, self.s_sub, self.s_absv = z3(), z3(), z3(), z3(), z3()
-        self.sw, self.w_eps, self.n_sub = z2(), z2(), z2()
-        self.pos = [int(p) for p in pos]
-        for t in range(T):
-            b, n = t // tps, self.pos[t] + 1
-            for g in range(Hkv):
-                hs = slice(g * r, (g + 1) * r)
-                qq, kk, vv = q[t, hs].double(), k[b, g, :n].double(), v[b, g, :n].double()
-                tl = (qq @ kk.T) * C_LOG2
-                tmax = tl.max(-1, keepdim=True).values
-                w = torch.exp2(tl - tmax)
-                sw = w.sum(-1)
-                o = (w @ vv) / sw[:, None]
-                dlt = C_ACC * C_LOG2 * (qq.abs() @ kk.abs().T) + 16 * U * torch.maximum(tl.abs(), tmax.abs())
-                eps = torch.exp2(dlt) - 1 + 2.0 ** -11
-                sub = (w < 2.0 ** -13).double()
-                dev = (vv[None] - o[:, None]).abs()
-                self.out[t, hs], self.sw[t, hs] = o, sw
-                self.s_eps[t, hs] = torch.einsum("rn,rnd->rd", w * eps, dev)
-                self.s_dev[t, hs] = torch.einsum("rn,rnd->rd", w, dev)
-                self.s_sub[t, hs] = torch.einsum("rn,rnd->rd", sub, dev)
-                self.s_absv[t, hs] = w @ vv.abs()
-                self.w_eps[t, hs], self.n_sub[t, hs] = (w * eps).sum(-1), sub.sum(-1)
-
-    def tol(self, tpw, n_split):
-        """tpw: tiles per warp of every token (list)."""
-        tw = torch.tensor(tpw, dtype=torch.float64, device=DEV).view(-1, 1)
-        ec = (tw + 3) * EXP2_REL
-        den = self.sw - self.w_eps - ec * self.sw - 2.0 ** -25 * self.n_sub
-        assert bool((den > 0).all())
-        p_err = (2 * (self.s_eps + ec[..., None] * self.s_dev) + 2 * 2.0 ** -25 * self.s_sub) / den[..., None]
-        acc = ((C_ACC + (tw[..., None] + n_split + 8) * U) * self.s_absv / self.sw[..., None]
-               + (5 * tw[..., None] + n_split // 32 + 20) * U * self.out.abs())
-        return (p_err + acc) * (1 + 2.0 ** -11) + 2.0 ** -11 * self.out.abs() + 2.0 ** -25
-
-    def ratio(self, out, n_split, chunk, even):
-        assert bool(torch.isfinite(out).all()), "non-finite output"
-        tpw = [_tpw(p + 1, n_split, chunk, even) for p in self.pos]
-        return float(((out.double() - self.out).abs() / self.tol(tpw, n_split)).max())
 
 
 def _regime(name, q0, k0):

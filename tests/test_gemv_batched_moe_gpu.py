@@ -49,13 +49,15 @@ import llama2_accessory_b200 as pkg  # noqa: E402
 from llama2_accessory_b200 import kvlayout, ops, quant  # noqa: E402
 from llama2_accessory_b200.engine import DecodeEngine, EngineConfig, _interleave_w13, rope_table  # noqa: E402
 from oracle.numerics import SENT, fp16_sides, kernel_route, nan16, tuned, x_candidates  # noqa: E402
+# the float64 checkers (bounds derived above) live in oracle/numerics.py, shared with test_engine_launch_audit_gpu.py
+from oracle.numerics import C_ACC, MAX_AMB, SILU_REL  # noqa: E402
+from oracle.numerics import gemv_check as _check, logit_window as _logit_window, rope_rotate as _rot  # noqa: E402
+from oracle.numerics import route_check as _route_check, route_scores32 as _scores32  # noqa: E402
+from oracle.numerics import silu_mul_range as _silu_mul_range  # noqa: E402
 
 DEV = "cuda"
 EPS = 1e-5
-C_ACC = 2.0 ** -18       # fp32 accumulation constant relative to M (see above)
 PROBE_MID = 2.0 ** -20   # sparse probes: skip outputs whose float64 value lies this close (relative) to an fp16 midpoint
-SILU_REL = 2.0 ** -20    # fp32 a / (1 + expf(-a)): <= 3.5 u << 16 u (test_decode_path_gpu.py)
-MAX_AMB = 12             # router: at most 2^12 rounding choices of ambiguous logits per token
 SLOT = 16384             # bytes of one weight-ring stage
 TS = [2, 3, 4, 5, 7, 8, 9, 15, 16, 17, 31, 32]
 
@@ -138,19 +140,6 @@ def _linear(bits, gs, N, K, seed, w13=False):
     zd = z.double().repeat_interleave(K // G, dim=1)
     qd = q.double()
     return pl, (qd - zd) * sd, sd * (qd + zd.abs())
-
-
-def _check(out, ref, M, label):
-    """out [T, N] against float64 ref with the section A bound -> (worst err / tol, implied C, exact fraction)."""
-    o = out.double()
-    assert torch.isfinite(o).all(), label
-    err = (o - ref).abs()
-    tol = ref.abs() * 2.0 ** -11 + C_ACC * M * (1 + 2.0 ** -10) + 2.0 ** -25
-    ratio = float((err / tol).max())
-    c_seen = float(((err - ref.abs() * 2.0 ** -11).clamp_min(0) / M.clamp_min(1e-30)).max())
-    exact = float((_bits16(out) == _bits16(ref.half())).double().mean())
-    assert ratio <= 1.0, (label, ratio)
-    return ratio, c_seen, exact
 
 
 def _gemv(pl, T, out, **kw):
@@ -361,14 +350,6 @@ def test_gemv_kernel_rmsnorm_and_silu_epilogue(gs):
     print(f"\n[rmsnorm+silu {gs or 'pc'}] " + "; ".join(rep))
 
 
-def _rot(y16, cs):
-    """fp32 RoPE as separate multiplies and adds: y16 [rows] fp16 of whole heads, cs [rows / 2, 2]."""
-    p = y16.float().reshape(-1, 2)
-    e, o = p[:, 0], p[:, 1]
-    c, s = cs[:, 0], cs[:, 1]
-    return torch.stack([e * c - o * s, e * s + o * c], dim=-1).reshape(-1).half()
-
-
 def _check_qkv(pl, W, A, Hq, Hkv, T, tps, p0, label, S=256):
     nq, nkv = Hq * 128, Hkv * 128
     nseq = -(-T // tps)
@@ -486,60 +467,6 @@ def _run_route(T, D, E, k, resid, delta, gamma, gate):
     return h_out, xn, sw[:-1].reshape(T, k), se[:-1].reshape(T, k)
 
 
-def _logit_window(xn, gate):
-    """float64 logits and the running-error bound R of the kernel's lane chains + warp tree (module docstring)."""
-    T, D = xn.shape
-    E = gate.shape[0]
-    p = xn.double()[:, None, :] * gate.double()[None]                       # [T, E, D] exact products
-    # lane l owns uint4 chunks u = l, l + 32, ...: elements 8u .. 8u + 7 in order
-    p = p.reshape(T, E, D // 256, 32, 8).permute(0, 1, 3, 2, 4).reshape(T, E, 32, D // 32)
-    part = p.cumsum(-1)
-    lane = part[..., -1]
-    R = 2.0 ** -24 * (part.abs().sum(-1).sum(-1) + 5 * lane.abs().sum(-1)) * (1 + 2.0 ** -10)
-    L = lane.sum(-1)
-    assert bool((R <= (D / 32 + 5) * 2.0 ** -24 * (xn.double().abs() @ gate.double().abs().T) * 1.01).all())
-    return L, R
-
-
-def _scores32(logits16):
-    lg = logits16.float().cpu().numpy()
-    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
-    den = np.zeros(lg.shape[0], dtype=np.float32)
-    for e in range(lg.shape[1]):
-        den = (den + ex[:, e]).astype(np.float32)
-    return torch.from_numpy((ex / den[:, None]).astype(np.float32)).double()
-
-
-def _route_check(xn, gate, sw, se, k):
-    """-> (tokens matched bit for bit, tokens in the expf window, tokens with too many ambiguous logits)."""
-    L, R = _logit_window(xn, gate)
-    near, alt, dist = fp16_sides(L)
-    amb = (dist <= R).cpu()
-    near, alt = near.cpu(), alt.cpu()
-    se_c, sw_c = se.cpu().long(), _bits16(sw).cpu()
-    matched = window = skipped = 0
-    for t in range(L.shape[0]):
-        ai = torch.nonzero(amb[t]).reshape(-1).tolist()
-        if len(ai) > MAX_AMB:
-            skipped += 1
-            continue
-        combos = torch.tensor(list(itertools.product([0, 1], repeat=len(ai))), dtype=torch.bool).reshape(2 ** len(ai), len(ai))
-        C = near[t].repeat(combos.shape[0], 1)
-        if ai:
-            C[:, ai] = torch.where(combos, alt[t, ai][None].expand_as(combos), near[t, ai][None].expand_as(combos))
-        lg16 = C.half()
-        idx, w = kernel_route(lg16, k)
-        hit = (idx == se_c[t][None]).all(1) & (w.view(torch.int16) == sw_c[t][None]).all(1)
-        if bool(hit.any()):
-            matched += 1
-            continue
-        s = _scores32(lg16)
-        _, _, sd = fp16_sides(s)
-        assert bool((sd <= 2.0 ** -20 * s.abs()).any()), (t, se_c[t].tolist(), idx[:4].tolist())
-        window += 1
-    return matched, window, skipped
-
-
 ROUTES = [(8, 2), (8, 1), (16, 4), (64, 8)]
 
 
@@ -616,26 +543,6 @@ def _ffn_weights(n_loc, gs, D, F, seed):
         w2.append(b[0])
         refs.append((a[1], a[2], b[1], b[2]))
     return w13, w2, refs
-
-
-SILU_ARGMIN = -1.2784645427610737  # silu has its only minimum there
-
-
-def _silu_mul_range(ya, ta, yb, tb):
-    """[lo, hi] of fp16(fp16(silu(a)) * b) over every fp16 a = fp16(y), |y - ya| <= ta (b likewise): fp16 rounding and
-    the product are monotone, silu is monotone on each side of its minimum, and the fp32 silu lies within SILU_REL."""
-    def silu(a):
-        return a / (1 + torch.exp(-a))
-    a_lo, a_hi = (ya - ta).half().double(), (ya + ta).half().double()
-    b_lo, b_hi = (yb - tb).half().double(), (yb + tb).half().double()
-    s1, s2 = silu(a_lo), silu(a_hi)
-    smin = torch.minimum(s1, s2)
-    smin = torch.where((a_lo <= SILU_ARGMIN) & (a_hi >= SILU_ARGMIN), torch.full_like(smin, silu(torch.tensor(SILU_ARGMIN, dtype=torch.float64)).item()), smin)
-    smax = torch.maximum(s1, s2)
-    s_lo = (smin - SILU_REL * smin.abs()).half().double()
-    s_hi = (smax + SILU_REL * smax.abs()).half().double()
-    c = torch.stack([s_lo * b_lo, s_lo * b_hi, s_hi * b_lo, s_hi * b_hi])
-    return c.amin(0).half().double(), c.amax(0).half().double()
 
 
 @pytest.mark.timeout(240)
