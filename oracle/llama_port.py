@@ -88,8 +88,9 @@ class PortModel:
         assert self.H % tp == 0 and self.Hkv % tp == 0
         self.k_cache = self.v_cache = None
         # diagnosis aids, both off by default: `record` (a list) receives one dict per forward_inference call with the
-        # residual stream after every block and the experts each token was routed to; `force_routes` maps
-        # (start_pos, layer) -> int64 [B * S, k] expert ids that MoE uses instead of its own top-k (in that slot order)
+        # residual stream after every block and after every block's attention, and the experts each token was routed to;
+        # `force_routes` maps (start_pos, layer) -> int64 [B * S, k] expert ids that MoE uses instead of its own top-k
+        # (in that slot order)
         self.record = None
         self.force_routes = None
         self._start_pos = 0
@@ -187,6 +188,8 @@ class PortModel:
     def block(self, i, x, start_pos, fc, causal):
         p = f"layers.{i}."
         h = x + self.attention(i, rmsnorm(x, self._w(p + "attention_norm.weight"), self.eps), start_pos, fc, causal)
+        if self.record is not None:
+            self.record[-1]["h_attn"].append(h.cpu().clone())
         n = rmsnorm(h, self._w(p + "ffn_norm.weight"), self.eps)
         return h + (self.ffn(i, n) if self.kind == "llama" else self.moe(i, n))
 
@@ -200,7 +203,7 @@ class PortModel:
         fc = self.freqs_cis[start_pos:start_pos + S]
         self._start_pos = start_pos
         if self.record is not None:
-            self.record.append(dict(start_pos=start_pos, h=[], routes=[], own=[], scores=[]))
+            self.record.append(dict(start_pos=start_pos, h=[], h_attn=[], routes=[], own=[], scores=[]))
         for i in range(self.L):
             h = self.block(i, h, start_pos, fc, causal=(S != 1))
             if self.record is not None:
