@@ -151,7 +151,8 @@ typedef struct {
    * a RowParallelLinear): the partial sums travel as 8-byte {half2, sequence number} units (the LL protocol of low-latency
    * collectives) through peer-mapped buffers of ar_world * N/2 units per rank.
    *   producer launch (wo / w2, EPI_F16): ar_out_peers = HOST array [ar_world] of the ranks' buffers; this rank's rows go to
-   *     slot ar_rank of EVERY buffer (`out` is not written);
+   *     slot ar_rank of EVERY buffer (`out` is not written), for every codec and both kernels (the integer-path gemv1 and
+   *     the generic HMMA kernel); not with MoE slot indirection;
    *   consumer launch (PRO_RMSNORM): ar_in = this rank's buffer; delta = sum over slots in rank order (fp32, one rounding).
    * sequence number = *ar_step * ar_period + id + 1: ar_step is a device counter the caller advances once per decode step,
    * ids distinguish the buffers' uses inside a step (< ar_period).  ar_error (optional, device u32) is set when a poll times

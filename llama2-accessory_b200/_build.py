@@ -9,7 +9,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = ["api.cu", "gemv.cu", "gemv1.cu", "mega1.cu", "mega2.cu", "attn.cu", "prefill.cu", "moe.cu", "sample.cu", "pack.cpp"]
-HDR = ["common.cuh", "gemv_core.cuh", "gemv1_core.cuh"]
+HDR = ["common.cuh", "gemv_core.cuh", "gemv1_core.cuh", "ll.cuh"]
 OUT = os.path.join(HERE, "libb200decode.so")
 STAMP = OUT + ".srchash"
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

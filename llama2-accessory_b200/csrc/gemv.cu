@@ -356,6 +356,11 @@ int b200::build_gemv_params(const b200_gemv_args_t* a, GemvParams* pp) {
         set_error("gemv: ar_out_peers needs the fp16 epilogue");
         return B200_E_INVAL;
       }
+      // every kernel pushes all N rows once; a MoE launch whose expert gets no routed token pushes nothing
+      if (a->slot_expert) {
+        set_error("gemv: ar_out_peers cannot be combined with MoE slot indirection");
+        return B200_E_INVAL;
+      }
       p.ll_out = 1;
       p.ll_out_id = a->ar_out_id;
       p.n_bcast = a->ar_world;

@@ -614,7 +614,20 @@ __device__ __forceinline__ void epilogue_role(const GemvParams& p, int T, const 
             const int r = r0 + 8 * hh, row = tile * 16 + r;
             const __half y16 = __float2half_rn(y[hh]);
             if (p.epi == B200_EPI_F16) {
-              if (col < T) reinterpret_cast<__half*>(p.out)[(size_t)(cols ? cols[col] : col) * p.N + row] = y16;
+              if (NT == 1 && p.ll_out) {
+                // fused all-reduce, push side (T == 1, so NT == 1 only: the larger instances carry no push code; as
+                // gemv1_core.cuh): rows r0 / r0 ^ 1 sit in lanes 8 apart; the shuffle runs on every lane, then the even
+                // row of column 0 stores {half2, seq} to every rank
+                const unsigned other = __shfl_xor_sync(0xffffffffu, (unsigned)__half_as_ushort(y16), 8);
+                if (col == 0 && (r0 & 1) == 0) {
+                  const unsigned pay = (unsigned)__half_as_ushort(y16) | (other << 16);
+                  const unsigned seq = *p.ll_step * (unsigned)p.ll_period + (unsigned)p.ll_out_id + 1u;
+                  for (int rr = 0; rr < p.n_bcast; ++rr)
+                    ll::ll_store(reinterpret_cast<uint8_t*>(p.bcast[rr]) + (size_t)(p.bcast_off + row) * 4, pay, seq);
+                }
+              } else if (col < T) {
+                reinterpret_cast<__half*>(p.out)[(size_t)(cols ? cols[col] : col) * p.N + row] = y16;
+              }
             } else if (p.epi == B200_EPI_F32) {
               if (col < T) {
                 if (p.n_bcast > 0) {  // vocabulary-sharded head: every rank receives this rank's slice of the logits

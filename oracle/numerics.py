@@ -4,8 +4,9 @@ split schedules and step-by-step arithmetic model of the decode attention kernel
 
 Also the float64 checkers that more than one GPU module applies (their bounds are derived in the docstrings of
 tests/test_gemv_batched_moe_gpu.py, sections A and B, and tests/test_attn_decode_gpu.py, section A): the GEMV bound,
-the RoPE of the QKV epilogue, the SiLU-product range, the router's logit window and routing check, and the float64
-reference and bound of decode attention.
+the RoPE of the QKV epilogue, the SiLU-product range, the router's logit window and routing check, the float64
+reference and bound of decode attention, and the LL unit format, sequence numbers and rank-sum model of the fused
+tensor-parallel all-reduce (tests/test_tp_allreduce_gpu.py derives its bound).
 
 Test infrastructure only (see oracle/__init__.py).  Every function here is plain torch / numpy; the CUDA library is only
 touched by `tuned`, and only when it is entered.
@@ -27,7 +28,7 @@ MAX_AMB = 12             # router: at most 2^12 rounding choices of ambiguous lo
 
 # what a b200_tune knob is when neither a b200_tune call nor the environment sets it (csrc: tune_get defaults)
 TUNE_DEFAULTS = {"B200_PF_EARLY": 0, "B200_SELF_PF_KB": 0, "B200_STREAM_EF": 1, "B200_QKV_RING_KB": 0, "B200_GEMV1": 1,
-                 "B200_ATTN_EVEN": 0, "B200_ATTN_MAX_SPLIT": 16, "B200_KV_EF": 1}
+                 "B200_GEMV1_GROUPED": 1, "B200_ATTN_EVEN": 0, "B200_ATTN_MAX_SPLIT": 16, "B200_KV_EF": 1}
 
 
 def nan16(*shape, device="cuda"):
@@ -384,3 +385,57 @@ class AttnRef:
         assert bool(torch.isfinite(out).all()), "non-finite output"
         tpw = [attn_tiles_per_warp(p + 1, n_split, chunk, even) for p in self.pos]
         return float(((out.double() - self.out).abs() / self.tol(tpw, n_split)).max())
+
+
+# ------------------------------------------------------------------- fused tensor-parallel all-reduce (ll.cuh) --------
+# An LL buffer holds [tp][N / 2] 8-byte units {payload, seq}: payload = fp16 bits of row 2j (low half) | row 2j + 1 (high
+# half) << 16, seq = the sequence number of the step that wrote it (tests/test_tp_allreduce_gpu.py derives the rank-sum
+# bound).  Units are numpy int32 [..., 2] here, as they lie in memory.
+LL_SENT = 0x7E5A7E5A     # one 32-bit word of two SENT halves: the sentinel of an LL buffer no kernel wrote
+
+
+def ll_seq(step, period, ident):
+    """The sequence number a launch stores / expects: (step * period + id + 1) mod 2^32, as uint32."""
+    return (int(step) * int(period) + int(ident) + 1) % (1 << 32)
+
+
+def ll_encode(parts16, seq):
+    """fp16 partials [tp, N] (numpy float16) -> int32 units [tp, N / 2, 2] carrying `seq`."""
+    bits = np.ascontiguousarray(parts16, dtype=np.float16).view(np.uint16).astype(np.uint32)
+    pay = bits[:, 0::2] | (bits[:, 1::2] << 16)
+    units = np.empty(pay.shape + (2,), dtype=np.uint32)
+    units[..., 0], units[..., 1] = pay, np.uint32(seq)
+    return units.view(np.int32)
+
+
+def ll_decode(units):
+    """int32 units [tp, N / 2, 2] -> (fp16 payloads [tp, N], uint32 sequence numbers [tp, N / 2])."""
+    u = np.ascontiguousarray(units).view(np.uint32)
+    pay, seq = u[..., 0], u[..., 1]
+    halves = np.stack([pay & 0xFFFF, pay >> 16], axis=-1).astype(np.uint16)
+    return halves.reshape(u.shape[0], -1).view(np.float16), seq
+
+
+def ll_rank_sum32(parts16, order=None):
+    """fp32 running sum of the partials [tp, N] (numpy float32), in rank order or in the given order of ranks."""
+    p = np.asarray(parts16, dtype=np.float16).astype(np.float32)
+    order = range(p.shape[0]) if order is None else order
+    acc = None
+    for r in order:
+        acc = p[r].copy() if acc is None else (acc + p[r]).astype(np.float32)
+    return acc
+
+
+def ll_rank_sum(parts16, order=None):
+    """The consumer's delta: the rank-order fp32 sum rounded once to fp16."""
+    return ll_rank_sum32(parts16, order).astype(np.float16)
+
+
+def ll_rank_sum_bound(parts16):
+    """-> (float64 exact sum s, bound) with |delta - s| <= 1/2 ulp16(s32) + (tp - 1) 2^-24 sum |p_r| (1 + 2^-20): tp - 1
+    fp32 additions, each off by at most 2^-24 of a partial sum bounded by sum |p_r| (up to its own rounding), then one
+    fp16 rounding of the fp32 sum s32 (half an fp16 spacing at |s32|; 2^-25 below the normal range)."""
+    p = np.asarray(parts16, dtype=np.float16).astype(np.float64)
+    s32 = np.abs(ll_rank_sum32(parts16).astype(np.float64))
+    half_ulp = 2.0 ** (np.floor(np.log2(np.maximum(s32, 2.0 ** -14))) - 11)
+    return p.sum(0), half_ulp + (p.shape[0] - 1) * 2.0 ** -24 * np.abs(p).sum(0) * (1 + 2.0 ** -20)

@@ -180,6 +180,9 @@ def test_malformed_arguments_are_refused_before_any_cuda_call():
         gemv(lin=plg, lin_group_size=96),                                       # group size that is not 64 / 128
         gemv(ar_world=2, ar_rank=0), gemv(ar_world=9, ar_rank=0, ar_step=x.data_ptr(), ar_period=4),
         gemv(T=2, ar_world=2, ar_rank=0, ar_step=x.data_ptr(), ar_period=4),    # fused all-reduce is bs = 1 only
+        # a push through MoE slot indirection: an expert with no routed token would push nothing
+        gemv(ar_world=2, ar_rank=0, ar_step=x.data_ptr(), ar_period=4, ar_out_peers=(C.c_void_p * 2)(x.data_ptr(), x.data_ptr()),
+             slot_expert=x.data_ptr(), n_slots=1),
     ]
     for rc, msg in bad:
         assert rc < 0 and msg, (rc, msg)
