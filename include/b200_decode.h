@@ -355,8 +355,10 @@ int b200_generate_update(const b200_generate_state_t* s, const int64_t* sampled,
 /* ------------------------------------------------------------------------------------------------
  * Mixtral top-2 MoE (mixtral.py:266-294).
  *   b200_moe_route: h = resid (+delta) -> h_out; xn = rmsnorm(h)*gamma -> xn_out fp16 [T,D];
- *     scores = softmax(gate xn) (fp16), top-k, renormalise; builds per-expert token lists for the
- *     writes, for slot (t, j) = t*topk + j:
+ *     logits = fp16(gate xn); scores = softmax(logits) in fp32, then by scores_f32:
+ *       0  scores rounded to fp16, top-k on them, renormalised in fp16            (mixtral.py:272-281)
+ *       1  top-k on the fp32 scores, fp32 sum, weight = fp16(score / sum)        (mixtral_sparse.py:417-428)
+ *     (top-k ties go to the lower expert index); writes, for slot (t, j) = t*topk + j:
  *       slot_expert  int32 [T*topk]       global expert id chosen for the slot
  *       slot_weight  fp16  [T*topk]       renormalised routing weight of the slot
  *     (the expert GEMVs scan slot_expert themselves: no atomics, deterministic column order)
@@ -374,6 +376,7 @@ typedef struct {
   void* slot_weight;  /* fp16 [T*topk] */
   int32_t* slot_expert; /* int32 [T*topk] */
   int use_pdl;
+  int scores_f32;     /* 0: fp16 score rule (mixtral), 1: fp32 score rule (mixtral_sparse); other values refused */
 } b200_moe_route_args_t;
 int b200_moe_route(const b200_moe_route_args_t* a, b200_stream_t stream);
 

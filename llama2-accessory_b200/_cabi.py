@@ -54,7 +54,7 @@ class MoeRouteArgs(C.Structure):
         ("T", C.c_int), ("D", C.c_int), ("E", C.c_int), ("topk", C.c_int),
         ("resid", C.c_void_p), ("delta", C.c_void_p), ("h_out", C.c_void_p), ("gamma", C.c_void_p),
         ("eps", C.c_float), ("gate_w", C.c_void_p), ("xn_out", C.c_void_p),
-        ("slot_weight", C.c_void_p), ("slot_expert", C.c_void_p), ("use_pdl", C.c_int),
+        ("slot_weight", C.c_void_p), ("slot_expert", C.c_void_p), ("use_pdl", C.c_int), ("scores_f32", C.c_int),
     ]
 
 

@@ -13,7 +13,9 @@ has no parameters to match against, so the tensor-parallel dimension of a tensor
     tp % ckpt_mp == 0 (:133-161), otherwise NotImplementedError (:164-168);
   * sharding dims (:34-38): ColumnParallelLinear weight dim 0, RowParallelLinear weight dim 1,
     ParallelEmbedding weight dim 1, everything else replicated; Mixtral experts live whole on the rank that
-    owns their id (mixtral.py:237-241);
+    owns their id (mixtral.py:237-241); ``mixtral_sparse`` stacks every expert's rows in one tensor per layer
+    and projection (``feed_forward.w1`` / ``w2`` / ``w3``, no ``.weight`` suffix, [E * F/TP, D] per rank) and
+    merges / splits it per expert (mixtral_sparse.py:210-219, 244-264);
   * ``meta.json`` / ``config.json`` / tokenizer probing of MetaModel.from_pretrained (meta.py:157-186,
     tokenizer.py:134-156).
 
@@ -42,6 +44,59 @@ _COLUMN = re.compile(r"(^|\.)(attention\.w[qkv]|feed_forward\.w[13]|output)\.wei
 _ROW = re.compile(r"(^|\.)(attention\.wo|feed_forward\.w2)\.weight$")
 _EMBED = re.compile(r"(^|\.)tok_embeddings\.weight$")
 _EXPERT = re.compile(r"(^|\.)feed_forward\.experts\.(\d+)\.w[123]\.weight$")
+# mixtral_sparse.py:244-264: one nn.Parameter per projection, [E * F_loc, D]; the keys carry no expert id, E is the
+# row count of the same layer's router (feed_forward.gate.weight [E, D], replicated on every rank)
+_SPARSE = re.compile(r"(^|\.)feed_forward\.w[123]$")
+
+
+def _sparse_gate_key(key: str) -> str:
+    return key[:-3] + ".gate.weight"
+
+
+def sparse_expert_merge(parts: Sequence[torch.Tensor], num_experts: int) -> torch.Tensor:
+    """Rank slices [E * F_r, D] of a sparse expert tensor -> [E * sum F_r, D] (mixtral_sparse.py:210-214)."""
+    return torch.cat([p.view(num_experts, -1, p.shape[-1]) for p in parts], dim=1).view(-1, parts[0].shape[-1]).contiguous()
+
+
+def sparse_expert_split(w: torch.Tensor, split_to: int, num_experts: int) -> List[torch.Tensor]:
+    """[E * F, D] -> split_to slices [E * F / split_to, D]: rows [r F/n, (r+1) F/n) of every expert
+    (mixtral_sparse.py:216-219, flattened the way the module's parameter holds them)."""
+    return [c.reshape(-1, w.shape[-1]).contiguous() for c in torch.chunk(w.view(num_experts, -1, w.shape[-1]), split_to, dim=1)]
+
+
+class SparseExpertView(Mapping):
+    """A mixtral_sparse state dict seen as per-expert linears: each ``layers.{i}.feed_forward.w{1,2,3}`` [E * F, D] becomes
+    ``layers.{i}.feed_forward.experts.{e}.w{1,2,3}.weight`` with w1 / w3 [F, D] (the expert's row block) and w2 [D, F] (the
+    transpose of its row block: the module applies x @ w2, mixtral_sparse.py:458).  Every other key passes through.  The
+    per-expert names are the base Mixtral ones, so quantisation, quant-record recovery and the engine's loader treat a
+    sparse checkpoint's experts as ordinary linears; the down projection is quantised as a [D, F] linear, groups along F."""
+
+    def __init__(self, sd: Mapping, num_experts: int):
+        self._sd, self._E = sd, num_experts
+        self._keys = OrderedDict()
+        for k in sd:
+            if _SPARSE.search(k):
+                for e in range(num_experts):
+                    self._keys[f"{k[:-3]}.experts.{e}.{k[-2:]}.weight"] = (k, e)
+            else:
+                self._keys[k] = (k, None)
+
+    def __len__(self):
+        return len(self._keys)
+
+    def __iter__(self):
+        return iter(self._keys)
+
+    def __contains__(self, key):
+        return key in self._keys
+
+    def __getitem__(self, key):
+        raw, e = self._keys[key]
+        w = self._sd[raw]
+        if e is None:
+            return w
+        blk = w.view(self._E, -1, w.shape[-1])[e]
+        return blk.t().contiguous() if raw.endswith("w2") else blk.contiguous()
 
 
 def get_tensor_parallel_shards_file_name(format: str, mp_size: int) -> List[str]:
@@ -126,10 +181,13 @@ def load_tensor_parallel_state_dict(path: str, tp_rank: int = 0, tp_world: int =
         shards = [load_tensor_parallel_shard_state_dict(path, format, s, ckpt_mp)
                   for s in range(n_local * tp_rank, n_local * (tp_rank + 1))]
         keys = list(OrderedDict.fromkeys(k for sh in shards for k in sh))
+        n_sparse = {k: shards[0][_sparse_gate_key(k)].shape[0] for k in keys if _SPARSE.search(k)}
         for key in keys:
             parts = [sh[key] for sh in shards if key in sh]
             dim = weight_parallel_dim(key)
-            if dim is not None:
+            if key in n_sparse:
+                out[key] = sparse_expert_merge(parts, n_sparse[key]) if len(parts) > 1 else parts[0]
+            elif dim is not None:
                 out[key] = torch.cat(parts, dim=dim) if len(parts) > 1 else parts[0]
             else:
                 if verbose and any(not torch.equal(parts[0], p) for p in parts[1:]):
@@ -144,6 +202,9 @@ def load_tensor_parallel_state_dict(path: str, tp_rank: int = 0, tp_world: int =
         split_id = tp_rank % split_to
         n_exp = None
         for key, val in shard.items():
+            if _SPARSE.search(key):
+                out[key] = sparse_expert_split(val, split_to, shard[_sparse_gate_key(key)].shape[0])[split_id]
+                continue
             e = _expert_id(key)
             if e is not None:
                 # this checkpoint rank holds a contiguous id range of whole experts; hand each new rank its slice
@@ -195,6 +256,8 @@ class LazyMergedStateDict(Mapping):
     def __getitem__(self, key):
         raw = self._raw[key]
         parts = [sh[raw] for sh in self._shards if raw in sh]
+        if _SPARSE.search(raw) and len(parts) > 1:
+            return sparse_expert_merge(parts, self._shards[0][_sparse_gate_key(raw)].shape[0])
         dim = weight_parallel_dim(raw)
         if dim is not None and len(parts) > 1:
             return torch.cat(parts, dim=dim)
@@ -252,7 +315,8 @@ def save_tensor_parallel_shards(master_sd: Dict[str, torch.Tensor], path: str, m
                                 wrap_model: bool = True) -> List[str]:
     """Write a TP = 1 state dict as an `mp_size`-way checkpoint folder in one of the reference's formats
     (the layout misc.py's save path produces: every rank holds its Column / Row / Embedding slice, replicated
-    tensors in every file, Mixtral experts in the file of the owning rank)."""
+    tensors in every file, Mixtral experts in the file of the owning rank, mixtral_sparse experts sliced over every
+    file)."""
     os.makedirs(path, exist_ok=True)
     n_exp = _num_experts(master_sd.keys())
     if n_exp and n_exp % mp_size:
@@ -263,7 +327,9 @@ def save_tensor_parallel_shards(master_sd: Dict[str, torch.Tensor], path: str, m
         for key, val in master_sd.items():
             k = key[5:] if key.startswith("llma.") else key
             e = _expert_id(k)
-            if e is not None:
+            if _SPARSE.search(k):
+                piece = sparse_expert_split(val, mp_size, master_sd[_sparse_gate_key(key)].shape[0])[r]
+            elif e is not None:
                 per = n_exp // mp_size
                 if not (per * r <= e < per * (r + 1)):
                     continue
@@ -391,10 +457,13 @@ def recover_quant_from_fake(w16: torch.Tensor, bits: int, group_size: int = 0):
 def recover_quant_records(sd: Dict[str, torch.Tensor], bits: int, group_size: int = 0, check: bool = True) -> Dict[str, dict]:
     """quant_records for DecodeEngine.load_master_state_dict from a fake-quantised MASTER state dict: every
     attention / feed-forward / expert linear (embeddings, norms, the lm_head and the MoE router stay fp16,
-    SURVEY.md 8c)."""
+    SURVEY.md 8c).  A mixtral_sparse state dict goes through SparseExpertView first: its records are per expert, the down
+    projection's along its input axis F."""
     recs = {}
     for key, w in sd.items():
         k = key[5:] if key.startswith("llma.") else key
+        if _SPARSE.search(k):
+            raise ValueError(f"{key}: stacked mixtral_sparse experts; pass SparseExpertView(sd, num_experts)")
         if not QUANTISED_KEY.search(k):
             continue
         q, s, z, g = recover_quant_from_fake(w, bits, group_size)
@@ -455,8 +524,9 @@ def load_packed(engine, path: str):
     if blob.get("version") != PACKED_FORMAT_VERSION:
         raise ValueError(f"packed shard version {blob.get('version')} != {PACKED_FORMAT_VERSION}")
     mine, theirs = asdict(c), blob["config"]
+    theirs = dict({"sparse_moe": False}, **theirs)  # shards written before mixtral_sparse existed: base Mixtral
     for k in ("kind", "dim", "n_layers", "n_heads", "n_kv_heads", "ffn_hidden", "vocab_size", "num_experts",
-              "experts_per_tok", "bits", "group_size", "tp_rank", "tp_world"):
+              "experts_per_tok", "bits", "group_size", "tp_rank", "tp_world", "sparse_moe"):
         if mine[k] != theirs[k]:
             raise ValueError(f"packed shard was written for {k}={theirs[k]}, engine has {k}={mine[k]}")
     dev = engine.device
@@ -476,7 +546,8 @@ def load_packed(engine, path: str):
 # ---------------------------------------------------------------------------------------------------
 # one call: checkpoint folder(s) -> engine
 # ---------------------------------------------------------------------------------------------------
-_KIND_OF_TYPE = {"llama": "llama", "llama_b200": "llama", "mixtral": "mixtral", "mixtral_b200": "mixtral"}
+_KIND_OF_TYPE = {"llama": "llama", "llama_b200": "llama", "mixtral": "mixtral", "mixtral_b200": "mixtral",
+                 "mixtral_sparse": "mixtral_sparse", "mixtral_sparse_b200": "mixtral_sparse"}
 
 
 def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, llama_type: Optional[str] = None,
@@ -500,7 +571,7 @@ def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, 
     if kind == "llama":  # defaults of llama.py:28-43
         for k, dflt in (("dim", 4096), ("n_layers", 32), ("n_heads", 32), ("multiple_of", 256), ("norm_eps", 1e-5)):
             args.setdefault(k, dflt)
-    else:  # defaults of mixtral.py:33-54
+    else:  # defaults of mixtral.py:33-54 (mixtral_sparse.py:47-68: the same)
         for k, dflt in (("dim", 4096), ("hidden_dim", 16384), ("n_layers", 32), ("n_heads", 32), ("norm_eps", 1e-5),
                         ("rope_theta", 1000000.0), ("moe", {"num_experts_per_tok": 2, "num_experts": 8})):
             args.setdefault(k, dflt)
@@ -511,9 +582,12 @@ def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, 
         # streaming: every linear is merged from the memory-mapped shards, quantised (or recovered), sharded, packed and
         # dropped before the next one is touched -- peak host memory is one merged tensor, not the master model
         sd = LazyMergedStateDict(paths[0], 0, 1)
-        recs = LazyQuantRecords(sd, bits, group_size) if (fake_quantised and bits != 16) else None
     else:  # base + *_diff chains need the accumulated values: eager
         sd = load_tensor_parallel_state_dict_list(paths, 0, 1)
-        recs = recover_quant_records(sd, bits, group_size) if (fake_quantised and bits != 16) else None
+    if kind == "mixtral_sparse":  # the stacked experts as per-expert linears, so that records are per expert
+        sd = SparseExpertView(sd, cfg.num_experts)
+    recs = None
+    if fake_quantised and bits != 16:
+        recs = (LazyQuantRecords if len(paths) == 1 else recover_quant_records)(sd, bits, group_size)
     eng.load_master_state_dict(sd, quant_records=recs)
     return eng, meta

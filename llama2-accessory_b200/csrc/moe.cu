@@ -1,4 +1,5 @@
-// Mixtral top-k MoE glue (accessory/model/LLM/mixtral.py:266-294): router, expert FFN driver, combine.
+// Mixtral top-k MoE glue (accessory/model/LLM/mixtral.py:266-294, mixtral_sparse.py:405-489): router, expert FFN
+// driver, combine.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -26,8 +27,12 @@ struct RouteParams {
   int* slot_expert;
 };
 
-// One CTA per token: residual add, RMSNorm (components.py:41-53), gate logits (fp16 F.linear),
-// softmax in fp32 -> fp16 (mixtral.py:275), top-k, renormalise in fp16 (mixtral.py:280).
+// One CTA per token: residual add, RMSNorm (components.py:41-53), gate logits (fp16 F.linear), then one of two score
+// rules:
+//   kScoresF32 = false (mixtral.py:272-281): softmax in fp32 -> fp16, top-k on the fp16 scores, renormalise in fp16;
+//   kScoresF32 = true  (mixtral_sparse.py:417-428): softmax in fp32, top-k on the fp32 scores, fp32 sum of the chosen
+//                      scores, weight = fp16(score / sum) rounded once.
+template <bool kScoresF32>
 __global__ void __launch_bounds__(kRouteThreads) moe_route_kernel(const __grid_constant__ RouteParams p) {
   extern __shared__ __align__(16) uint8_t smem[];
   __half* xs = reinterpret_cast<__half*>(smem);  // [D]
@@ -105,8 +110,11 @@ __global__ void __launch_bounds__(kRouteThreads) moe_route_kernel(const __grid_c
     float den = 0.f;
     for (int e = 0; e < p.E; ++e) den += expf(s_logit[e] - mx);
     float sc[kMaxExperts];
-    for (int e = 0; e < p.E; ++e) sc[e] = __half2float(__float2half_rn(expf(s_logit[e] - mx) / den));
-    // top-k on the fp16 scores; ties -> lowest index first
+    for (int e = 0; e < p.E; ++e) {
+      const float v = expf(s_logit[e] - mx) / den;
+      sc[e] = kScoresF32 ? v : __half2float(__float2half_rn(v));
+    }
+    // top-k on the scores (fp16-valued or fp32); ties -> lowest index first
     int idx[8];
     float val[8];
     for (int j = 0; j < p.topk; ++j) {
@@ -121,10 +129,11 @@ __global__ void __launch_bounds__(kRouteThreads) moe_route_kernel(const __grid_c
     }
     float sum = 0.f;
     for (int j = 0; j < p.topk; ++j) sum += val[j];
-    const float sum16 = __half2float(__float2half_rn(sum));  // fp16 .sum(dim=-1)
+    // fp16 rule: .sum(dim=-1) of a half tensor is rounded to fp16; fp32 rule: the sum stays fp32
+    const float den_k = kScoresF32 ? sum : __half2float(__float2half_rn(sum));
     for (int j = 0; j < p.topk; ++j) {
       p.slot_expert[t * p.topk + j] = idx[j];
-      p.slot_weight[t * p.topk + j] = __float2half_rn(val[j] / sum16);
+      p.slot_weight[t * p.topk + j] = __float2half_rn(val[j] / den_k);
     }
   }
 }
@@ -161,6 +170,10 @@ extern "C" int b200_moe_route(const b200_moe_route_args_t* a, b200_stream_t stre
     set_error("moe_route: unsupported shape");
     return B200_E_UNSUPPORTED;
   }
+  if (a->scores_f32 != 0 && a->scores_f32 != 1) {
+    set_error("moe_route: scores_f32 must be 0 (fp16 scores) or 1 (fp32 scores)");
+    return B200_E_INVAL;
+  }
   RouteParams p = {};
   p.T = a->T, p.D = a->D, p.E = a->E, p.topk = a->topk;
   p.resid = static_cast<const __half*>(a->resid);
@@ -182,7 +195,8 @@ extern "C" int b200_moe_route(const b200_moe_route_args_t* a, b200_stream_t stre
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = a->use_pdl ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, moe_route_kernel, p);
+  cudaError_t e = a->scores_f32 ? cudaLaunchKernelEx(&cfg, moe_route_kernel<true>, p)
+                                 : cudaLaunchKernelEx(&cfg, moe_route_kernel<false>, p);
   if (e != cudaSuccess) {
     set_error(std::string("moe_route: ") + cudaGetErrorString(e));
     return (int)e;

@@ -13,7 +13,10 @@ router -> per-expert gate/up + down -> weighted combine (mixtral.py:266-294).
 
 Tensor parallelism follows the reference (one process per GPU, column-parallel wq/wk/wv/w1/w3/output,
 row-parallel wo/w2, whole experts per rank, one all-reduce after each row-parallel linear); the
-collectives are NCCL calls on the same stream, captured in the same graph.
+collectives are NCCL calls on the same stream, captured in the same graph.  `mixtral_sparse` models
+(EngineConfig.sparse_moe) slice every expert instead: rank r holds rows [r F/TP, (r+1) F/TP) of every
+expert's w1 / w3 and the same input columns of its down projection (mixtral_sparse.py:222-264), and route
+with the fp32 score rule (mixtral_sparse.py:417-428).
 """
 import math
 import os
@@ -69,6 +72,8 @@ class EngineConfig:
     group_size: int = 0
     tp_rank: int = 0
     tp_world: int = 1
+    # mixtral_sparse: every rank holds 1/TP of every expert (ffn_hidden / TP rows), fp32 router scores
+    sparse_moe: bool = False
 
     @property
     def head_dim(self):
@@ -80,6 +85,9 @@ class EngineConfig:
 
     @classmethod
     def from_model_args(cls, kind, a: dict, **kw):
+        """kind: 'llama' | 'mixtral' | 'mixtral_sparse' (served as kind 'mixtral' with sparse_moe = True)."""
+        if kind == "mixtral_sparse":
+            kind, kw = "mixtral", dict(kw, sparse_moe=True)
         if kind == "llama":
             ffn = llama_ffn_hidden(a["dim"], a.get("multiple_of", 256), a.get("ffn_dim_multiplier"))
             theta = a.get("rope_theta", 10000.0)
@@ -135,7 +143,10 @@ def check_kernel_limits(cfg: "EngineConfig"):
     tp = max(1, cfg.tp_world)
     if cfg.dim % 128 or cfg.dim > 8192:
         raise ValueError(f"dim = {cfg.dim}: the fused RMSNorm prologue takes multiples of 128 up to 8192")
-    f_loc = cfg.ffn_hidden // tp if cfg.kind == "llama" else cfg.ffn_hidden
+    f_loc = cfg.ffn_hidden // tp if (cfg.kind == "llama" or cfg.sparse_moe) else cfg.ffn_hidden
+    if cfg.sparse_moe and (cfg.ffn_hidden % tp or f_loc % 128):
+        # mixtral_sparse.py:333: the expert slices are whole 128-row blocks (and the engine pads no expert)
+        raise ValueError(f"mixtral_sparse: hidden_dim / TP = {cfg.ffn_hidden} / {tp} must be a multiple of 128")
     if (f_loc + 127) // 128 * 128 > 16384:
         raise ValueError(f"local FFN width {f_loc} > 16384: shard the model over more tensor-parallel ranks "
                          f"(tp_world = {tp}; LLaMA2-70B needs TP >= 2)")
@@ -162,12 +173,14 @@ class DecodeEngine:
         self.group = group
         self.Hq = cfg.n_heads // cfg.tp_world
         self.Hkv = cfg.kv_heads // cfg.tp_world
-        self.F_raw = cfg.ffn_hidden // cfg.tp_world if cfg.kind == "llama" else cfg.ffn_hidden
+        self.F_raw = cfg.ffn_hidden // cfg.tp_world if (cfg.kind == "llama" or cfg.sparse_moe) else cfg.ffn_hidden
         # the GEMV streams K in 64..128-wide blocks: pad the local FFN width (e.g. 11008/8 = 1376 -> 1408) with
         # zero weights (rows of w1/w3, columns of w2); the padded activations are exactly 0
         self.F = (self.F_raw + 127) // 128 * 128
         self.V_loc = cfg.vocab_size // cfg.tp_world
-        if cfg.kind == "mixtral":
+        if cfg.kind == "mixtral" and cfg.sparse_moe:  # every expert, F_raw of its rows
+            self.E_loc, self.e_first = cfg.num_experts, 0
+        elif cfg.kind == "mixtral":
             assert cfg.num_experts % cfg.tp_world == 0
             self.E_loc = cfg.num_experts // cfg.tp_world
             self.e_first = self.E_loc * cfg.tp_rank
@@ -309,7 +322,8 @@ class DecodeEngine:
 
     def load_local_state_dict(self, sd: dict):
         """sd: this rank's shards, exactly what accessory/util/tensor_parallel.py hands to load_state_dict
-        (Column [out/TP, in], Row [out, in/TP], Embedding [vocab, D/TP], local experts only).  Quantisation
+        (Column [out/TP, in], Row [out, in/TP], Embedding [vocab, D/TP], local experts only; mixtral_sparse: w1 / w2 / w3
+        [E * F/TP, D], rank r's rows of every expert).  Quantisation
         is rank-local min/max (DESIGN.md: differs from quantise-master-then-shard only for row-parallel
         per-channel scales)."""
         return self.load_master_state_dict(sd, None, _sharded=True)
@@ -317,7 +331,11 @@ class DecodeEngine:
     def load_master_state_dict(self, sd: dict, quant_records: Optional[dict] = None, _sharded=False):
         """sd: MASTER (TP=1) fp16 state dict, keys as in SURVEY.md 8b (optionally prefixed 'llma.').
         quant_records: optional {key: dict(q, scale, zero, group_size)} for the quantised linears of the
-        master model (e.g. recovered from an OmniQuant checkpoint); otherwise quantised here."""
+        master model (e.g. recovered from an OmniQuant checkpoint); otherwise quantised here.
+        mixtral_sparse (cfg.sparse_moe): the stacked w1 / w2 / w3 [E * F, D] are read through checkpoint.SparseExpertView,
+        i.e. as the per-expert linears experts.{e}.w1 / w3 [F, D] and w2 [D, F] (the transpose of the stored row block,
+        mixtral_sparse.py:458); quant_records are keyed by those per-expert names.  Each is quantised whole and then
+        sliced like a column- (w1, w3) or row-parallel (w2) linear, so no group straddles a slice."""
         c = self.cfg
         col, row = ("none", "none") if _sharded else ("col", "row")
         # plain dicts are re-keyed without the 'llma.' prefix; lazy mappings (checkpoint.LazyMergedStateDict / LazyQuantRecords:
@@ -326,6 +344,10 @@ class DecodeEngine:
             sd = {(k[5:] if k.startswith("llma.") else k): v for k, v in sd.items()}
         if isinstance(quant_records, dict):
             quant_records = {(k[5:] if k.startswith("llma.") else k): v for k, v in quant_records.items()}
+        if c.sparse_moe:
+            from .checkpoint import SparseExpertView
+            if not isinstance(sd, SparseExpertView):
+                sd = SparseExpertView(sd, c.num_experts)
         bits, gs, dev = c.bits, c.group_size, self.device
         emb = sd["tok_embeddings.weight"].to(torch.float16).to(dev).contiguous()
         if _sharded and c.tp_world > 1:  # [vocab, D/TP] shards -> full replicated table
@@ -352,11 +374,12 @@ class DecodeEngine:
                 lw.w2 = self._make_linear(p + "feed_forward.w2.weight", sd, quant_records, bits, gs, row, pad_cols=fpad)
             else:
                 lw.gate = sd[p + "feed_forward.gate.weight"].to(torch.float16).to(dev).contiguous()
+                ecol, erow = (col, row) if c.sparse_moe else ("none", "none")
                 for e in range(self.e_first, self.e_first + self.E_loc):
                     q = p + f"feed_forward.experts.{e}."
-                    lw.e_w13.append(self._make_linear(q + "w1.weight", sd, quant_records, bits, gs, "none",
+                    lw.e_w13.append(self._make_linear(q + "w1.weight", sd, quant_records, bits, gs, ecol,
                                                       interleave_with=q + "w3.weight"))
-                    lw.e_w2.append(self._make_linear(q + "w2.weight", sd, quant_records, bits, gs, "none"))
+                    lw.e_w2.append(self._make_linear(q + "w2.weight", sd, quant_records, bits, gs, erow))
         return self
 
     def load_random(self, seed=0):
@@ -515,7 +538,8 @@ class DecodeEngine:
                 k = c.experts_per_tok
                 ops.moe_route(T=T, D=c.dim, E=c.num_experts, topk=k, resid=self.h[cur], delta=self.o,
                               h_out=self.h[1 - cur], gamma=lw.ffn_norm, eps=c.norm_eps, gate_w=lw.gate,
-                              xn_out=self.xn, slot_weight=self.slot_w, slot_expert=self.slot_e, use_pdl=pdl)
+                              xn_out=self.xn, slot_weight=self.slot_w, slot_expert=self.slot_e, use_pdl=pdl,
+                              scores_f32=c.sparse_moe)
                 cur = 1 - cur
                 ops.moe_expert_ffn(lw.e_w13, lw.e_w2, T=T, D=c.dim, F=self.F, topk=k, e_first=self.e_first,
                                    xn=self.xn, slot_expert=self.slot_e, act=self.act_slots, y_slot=self.y_slot,
@@ -726,7 +750,7 @@ class DecodeEngine:
                 ns, fe = T * k, lw.e_w2[0].K  # fe: the experts' own FFN width (they are not padded to self.F)
                 ops.moe_route(T=T, D=c.dim, E=c.num_experts, topk=k, resid=b["h"][cur], delta=b["o"], h_out=b["h"][1 - cur],
                               gamma=lw.ffn_norm, eps=c.norm_eps, gate_w=lw.gate, xn_out=b["x"], slot_weight=b["slot_w"],
-                              slot_expert=b["slot_e"])
+                              slot_expert=b["slot_e"], scores_f32=c.sparse_moe)
                 cur = 1 - cur
                 ops.prefill_moe_gemm_w4(lw.e_w13, b["x"], b["gu"], slot_expert=b["slot_e"], n_slots=ns, src_div=k,
                                         e_first=self.e_first)

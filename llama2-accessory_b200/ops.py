@@ -232,7 +232,9 @@ def generate_update(state, sampled):
 
 
 def moe_route(*, T, D, E, topk, resid, delta, h_out, gamma, eps, gate_w, xn_out, slot_weight, slot_expert,
-              use_pdl=False):
+              use_pdl=False, scores_f32=False):
+    """scores_f32: top-k and renormalisation on the fp32 softmax scores (mixtral_sparse.py:417-428) instead of the
+    fp16-rounded ones (mixtral.py:272-281)."""
     global launch_count
     a = _cabi.MoeRouteArgs()
     a.T, a.D, a.E, a.topk = T, D, E, topk
@@ -240,6 +242,7 @@ def moe_route(*, T, D, E, topk, resid, delta, h_out, gamma, eps, gate_w, xn_out,
     a.eps = eps
     a.gate_w, a.xn_out, a.slot_weight, a.slot_expert = _p(gate_w), _p(xn_out), _p(slot_weight), _p(slot_expert)
     a.use_pdl = int(use_pdl)
+    a.scores_f32 = int(scores_f32)
     _cabi.check(_cabi.lib().b200_moe_route(C.byref(a), _stream()), "b200_moe_route")
     launch_count += 1
 
