@@ -328,8 +328,10 @@ int b200_advance_pos(int32_t* pos, int T, int inc, b200_stream_t stream);
 /* next[t] ~ top-p(softmax(logits[t] / temperature)):  a token is kept iff the probabilities strictly larger than
  * its own sum to <= top_p (the reference's "cumsum - p > top_p" mask; equal probabilities are kept or dropped
  * together), the kept set is renormalised and sampled by inverse CDF in index order with uniform[t] in [0, 1).
- * temperature and top_p must be > 0 (temperature 0 is b200_argmax, meta.py:441-442).  One CTA per row, the V
- * probabilities live in shared memory (V <= ~57000). */
+ * temperature and top_p must be > 0 (temperature 0 is b200_argmax, meta.py:441-442).  One CTA per row, any V >= 1.
+ * While the V fp32 probabilities fit in shared memory (V <= 57856 with the H100's 227 KB opt-in) they are held there and
+ * the threshold is bisected; a larger vocabulary re-reads the logits row (L2-resident) on every pass and finds the
+ * threshold by a 4-pass radix descent with the masses summed in 2^-56 fixed point.  No workspace either way. */
 int b200_sample_top_p(const float* logits, const float* uniform, int64_t* next, int T, int V, float temperature,
                       float top_p, b200_stream_t stream);
 

@@ -145,6 +145,157 @@ sample_top_p_kernel(const float* __restrict__ logits, const float* __restrict__ 
   if (tid == 0) next[t] = s_tok < 0 ? 0 : s_tok;
 }
 
+// Top-p sampling for vocabularies whose probabilities do not fit in shared memory (V > ~57800 on the H100): the same
+// rule and the same draw as sample_top_p_kernel, with nothing stored per token.  Every pass re-reads the logits row
+// (L2-resident: 412 KB at V = 103168) and recomputes p_i = exp((l_i - max) / T) / sum, bit for bit the value the other
+// kernel keeps in shared memory.  The threshold is found by a radix descent on the bit pattern of p (4 passes of 8 bits,
+// most significant first) instead of 30 bisection passes: each pass histograms the probability mass of the tokens that
+// share the prefix fixed so far, and keeps the lowest non-empty bin whose largest member still has at most top_p of
+// mass strictly above it.  The masses are summed in 2^-56 fixed point (exact for every p >= 2^-33; a smaller p counts
+// as 2^-56), so the integer atomics are order-independent and the cut is the same on every run.  A 64-bit sum is kept as
+// two 32-bit words with the carry taken from the low word's atomic: shared-memory atomics are native at 32 bits, while a
+// 64-bit add is a compare-and-swap loop that spins under the contention of a whole vocabulary landing in a few bins.
+constexpr int kRadixBins = 256;
+constexpr float kFix = 72057594037927936.0f;  // 2^56
+
+__device__ __forceinline__ unsigned long long fixed_mass(float p) {
+  const unsigned long long f = __float2ull_rz(p * kFix);
+  return f ? f : 1ull;  // p > 0 always counts, so a bin is non-empty iff its mass is
+}
+
+__device__ __forceinline__ void add_mass(unsigned* lo, unsigned* hi, unsigned long long v) {
+  const unsigned vl = (unsigned)v, vh = (unsigned)(v >> 32);
+  const unsigned old = atomicAdd(lo, vl);
+  const unsigned up = vh + (old + vl < old ? 1u : 0u);  // + the carry out of the low word
+  if (up) atomicAdd(hi, up);
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+sample_top_p_radix_kernel(const float* __restrict__ logits, const float* __restrict__ u, long long* __restrict__ next,
+                          int V, float inv_temperature, float top_p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ unsigned hist_lo[kRadixBins], hist_hi[kRadixBins];
+  __shared__ float red[kSampleThreads / 32];
+  __shared__ float wtot[kSampleThreads / 32];
+  __shared__ unsigned s_prefix;
+  __shared__ unsigned long long s_above;
+  __shared__ int s_tok;
+  const int t = blockIdx.x, tid = threadIdx.x;
+  const float* row = logits + (size_t)t * V;
+
+  float m = -INFINITY;
+  for (int i = tid; i < V; i += kSampleThreads) m = fmaxf(m, row[i]);
+  m = block_max(m, red);
+  float s = 0.f;
+  for (int i = tid; i < V; i += kSampleThreads) s += expf((row[i] - m) * inv_temperature);
+  s = block_sum(s, red);
+  const float inv = 1.0f / s;
+  const auto prob = [&](int i) { return expf((row[i] - m) * inv_temperature) * inv; };
+
+  unsigned prefix = 0u;  // bit pattern of the cut, fixed from the top down
+  if (top_p < 1.0f) {
+    const unsigned long long limit = __float2ull_rz(top_p * kFix);
+    unsigned long long above = 0ull;  // mass of the tokens whose pattern is above every pattern with this prefix
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      if (tid < kRadixBins) hist_lo[tid] = hist_hi[tid] = 0u;
+      __syncthreads();
+      const unsigned fixed = shift == 24 ? 0u : ~0u << (shift + 8);
+      for (int i = tid; i < V; i += kSampleThreads) {
+        const float p = prob(i);
+        const unsigned b = __float_as_uint(p);
+        const int d = (b >> shift) & (kRadixBins - 1);
+        if (p > 0.f && (b & fixed) == prefix) add_mass(&hist_lo[d], &hist_hi[d], fixed_mass(p));
+      }
+      __syncthreads();
+      if (tid < 32) {
+        // lane l owns bins [8l, 8l + 8); mass of the bins above lane l's = suffix sum over the higher lanes
+        unsigned long long h[8], own = 0ull;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) own += (h[j] = (unsigned long long)hist_hi[8 * tid + j] << 32 | hist_lo[8 * tid + j]);
+        unsigned long long higher = own;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const unsigned long long v = __shfl_down_sync(0xffffffffu, higher, o);
+          if (tid + o < 32) higher += v;
+        }
+        unsigned long long a = above + higher - own;  // mass above bin 8l + 7
+        int bin = -1;
+        unsigned long long bin_above = 0ull;
+#pragma unroll
+        for (int j = 7; j >= 0; --j) {
+          if (h[j] && a <= limit) { bin = 8 * tid + j; bin_above = a; }
+          a += h[j];
+        }
+        // the lowest qualifying bin: masses above grow towards lower bins, so the qualifying lanes are the upper ones
+        const unsigned have = __ballot_sync(0xffffffffu, bin >= 0);
+        if (have && tid == __ffs(have) - 1) {
+          s_prefix = prefix | ((unsigned)bin << shift);
+          s_above = bin_above;
+        }
+      }
+      __syncthreads();
+      prefix = s_prefix;
+      above = s_above;
+    }
+  }
+
+  // inverse CDF over the kept tokens in index order, as in sample_top_p_kernel: thread tid owns the chunk [c0, c1)
+  const float cut = __uint_as_float(prefix);  // keep p_i >= cut
+  const int chunk = (V + kSampleThreads - 1) / kSampleThreads;
+  const int c0 = min(V, tid * chunk), c1 = min(V, c0 + chunk);
+  float part = 0.f;
+  for (int i = c0; i < c1; ++i) {
+    const float p = prob(i);
+    if (p >= cut && p > 0.f) part += p;
+  }
+  // block-wide exclusive scan of the chunk sums (warp scan, then scan of the 32 warp totals)
+  float incl = part;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float v = __shfl_up_sync(0xffffffffu, incl, o);
+    if ((tid & 31) >= o) incl += v;
+  }
+  if ((tid & 31) == 31) wtot[tid >> 5] = incl;
+  if (tid == 0) s_tok = -1;
+  __syncthreads();
+  float base = 0.f, total = 0.f;
+#pragma unroll
+  for (int w = 0; w < kSampleThreads / 32; ++w) {
+    if (w < (tid >> 5)) base += wtot[w];
+    total += wtot[w];
+  }
+  const float excl = base + incl - part;
+  const float target = u[t] * total;
+  if (part > 0.f && excl <= target && target < excl + part) {
+    float acc = excl;
+    int pick = -1;
+    for (int i = c0; i < c1; ++i) {
+      const float p = prob(i);
+      if (p >= cut && p > 0.f) {
+        pick = i;
+        acc += p;
+        if (target < acc) break;
+      }
+    }
+    s_tok = pick;
+  }
+  __syncthreads();
+  const bool unclaimed = s_tok < 0;  // read by everybody before anybody may write again
+  __syncthreads();
+  if (unclaimed) {
+    // u * total rounded onto (or past) the end of the last interval: take the last kept token
+    int last = -1;
+    for (int i = c1 - 1; i >= c0; --i) {
+      const float p = prob(i);
+      if (p >= cut && p > 0.f) { last = i; break; }
+    }
+    if (last >= 0) atomicMax(&s_tok, last);
+  }
+  __syncthreads();
+  if (tid == 0) next[t] = s_tok < 0 ? 0 : s_tok;
+}
+
 // One thread per sequence: meta.py:446-461 for position cur = *cur_pos.
 //   forced token while the position is still inside the sequence's own prompt (input_text_mask, :446-448),
 //   tokens[:, cur] = next (:449), stop bookkeeping in the reference's order (:451-459: first matching stop sequence
@@ -211,8 +362,15 @@ extern "C" int b200_sample_top_p(const float* logits, const float* uniform, int6
   }
   const size_t smem = (size_t)V * sizeof(float);
   if (smem + 1024 > smem_optin()) {
-    set_error("sample_top_p: vocabulary does not fit in shared memory");
-    return B200_E_UNSUPPORTED;
+    // the probabilities do not fit in shared memory: recompute them from the logits row on every pass
+    sample_top_p_radix_kernel<<<T, kSampleThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        logits, uniform, reinterpret_cast<long long*>(next), V, 1.0f / temperature, top_p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+      set_error(std::string("sample_top_p: ") + cudaGetErrorString(e));
+      return (int)e;
+    }
+    return 0;
   }
   static size_t configured_dev[16] = {};  // cudaFuncSetAttribute is per device
   int dev = 0;
