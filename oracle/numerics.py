@@ -431,6 +431,64 @@ def ll_rank_sum(parts16, order=None):
     return ll_rank_sum32(parts16, order).astype(np.float16)
 
 
+def ll_units_decode32(units):
+    """int32 LL units [..., 2] whose payload is an fp32 (the attention partials of mega2.cu) -> (float32 payloads, uint32
+    sequence numbers)."""
+    u = np.ascontiguousarray(units).view(np.uint32)
+    return u[..., 0].copy().view(np.float32), u[..., 1].copy()
+
+
+# ------------------------------------------------------------ persistent whole-step kernels (mega1.cu, mega2.cu) --------
+MEGA_TILE, MEGA_WARPS = 32, 16     # kv positions per attention tile, MMA warps per CTA (kTileKV, kConsumerWarps)
+
+
+def mega_split_ranges(kv_len, n_split):
+    """attn_item of mega1.cu / mega2.cu: [(s_begin, s_end)] of every split, equal chunks of whole 32-key tiles sized for
+    kv_len; s_end == s_begin is an empty split.  Tile i of a split belongs to MMA warp i % 16."""
+    chunk = _cdiv(_cdiv(kv_len, n_split), MEGA_TILE) * MEGA_TILE
+    return [(min(kv_len, sp * chunk), min(kv_len, (sp + 1) * chunk)) for sp in range(n_split)]
+
+
+def mega_tiles_per_warp(kv_len, n_split):
+    """largest number of tiles one MMA warp of the persistent kernels folds for one (kv head, split) item."""
+    return max(_cdiv(_cdiv(e - b, MEGA_TILE), MEGA_WARPS) for b, e in mega_split_ranges(kv_len, n_split))
+
+
+def mega_past_boundary_pos(n_split):
+    """A position whose kv_len = pos + 1 puts exactly one key into the last of n_split splits (chunk 32 n_split)."""
+    return MEGA_TILE * n_split * (n_split - 1)
+
+
+def mega1_comm_offsets(n_layers, dim, tp=1):
+    """(parts, logits) byte offsets of mega1's communication block: u32 counters [5L + 3] padded to 256 B, then fp16
+    partials [2][tp][dim] (wo | w2) padded to 256 B, then fp32 logits (b200_step1_comm_logits_offset)."""
+    bar = ((5 * n_layers + 3) * 4 + 255) // 256 * 256
+    return bar, bar + (2 * tp * dim * 2 + 255) // 256 * 256
+
+
+def ll_layout(n_layers, D, Hq, Hkv, F, V, n_split, tp=1):
+    """Byte offsets of mega2's communication block (make_layout): ctl | yq | ykv | att | po | act | pf | logits | total."""
+    al = lambda v: (v + 255) // 256 * 256  # noqa: E731
+    sizes = [("ctl", 64 + (5 * n_layers + 1) * 4), ("yq", Hq * 128 * 4), ("ykv", Hkv * 2 * 128 * 4),
+             ("att", Hq * n_split * 130 * 8), ("po", tp * D * 4), ("act", F * 4), ("pf", tp * D * 4), ("logits", V * tp * 4)]
+    off, out = 0, {}
+    for k, n in sizes:
+        out[k] = off
+        off = al(off + n)
+    out["total"] = off
+    return out
+
+
+def merge_splits64(O, m, lsum):
+    """float64 cross-split merge of per-split partials O [H, ns, 128], m, l [H, ns] (log2 units) -> [H, 128], and the
+    magnitude sum_sp |O_sp| f_sp / L that bounds the fp32 rounding of the kernels' own merge."""
+    O, m, lsum = O.double(), m.double(), lsum.double()
+    M = m.max(-1, keepdim=True).values
+    f = torch.where(torch.isinf(m), torch.zeros_like(m), torch.exp2(m - M))
+    L = (lsum * f).sum(-1, keepdim=True)
+    return (O * f[..., None]).sum(1) / L, (O.abs() * f[..., None]).sum(1) / L
+
+
 def ll_rank_sum_bound(parts16):
     """-> (float64 exact sum s, bound) with |delta - s| <= 1/2 ulp16(s32) + (tp - 1) 2^-24 sum |p_r| (1 + 2^-20): tp - 1
     fp32 additions, each off by at most 2^-24 of a partial sum bounded by sum |p_r| (up to its own rounding), then one
