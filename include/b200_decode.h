@@ -100,6 +100,11 @@ typedef struct {
  * ---------------------------------------------------------------------------------------------- */
 enum { B200_PRO_NONE = 0, B200_PRO_RMSNORM = 1 };
 enum { B200_EPI_F16 = 0, B200_EPI_F32 = 1, B200_EPI_QKV = 2, B200_EPI_SILU = 3 };
+/* Optional fp16 bias b[N] of the linear (InternLM's Wqkv / out_proj, internlm.py:75-89), two rounding points:
+ *   B200_BIAS_ACC  out = fp16(acc + b)           (fp32 add, one rounding: F.linear(x, W, b))
+ *   B200_BIAS_OUT  out = fp16(fp16(acc) + b)     (fp16 add of the rounded output: RowParallelLinear's y + bias)
+ * In EPI_QKV the bias is added before RoPE. */
+enum { B200_BIAS_NONE = 0, B200_BIAS_ACC = 1, B200_BIAS_OUT = 2 };
 
 typedef struct {
   b200_linear_t lin;
@@ -168,6 +173,10 @@ typedef struct {
    * miss queued behind its own weight stream.  NULL/0 = off.  bytes: multiple of 16. */
   const void* prefetch_const;
   int prefetch_const_bytes;
+  /* Optional bias (B200_BIAS_*): fp16 [N] with bias_mode 1 or 2; NULL with bias_mode 0.  EPI_F16 and EPI_QKV only; not with
+   * MoE slot indirection or ar_world > 1. */
+  const void* bias;
+  int bias_mode;
 } b200_gemv_args_t;
 
 int b200_gemv(const b200_gemv_args_t* a, b200_stream_t stream);
@@ -258,6 +267,10 @@ int b200_ipc_free(void* own_ptr);
  *   b200_prefill_silu_mul  gu [T][2F] (w1 / w3 interleaved 8 + 8 as for EPI_SILU) -> act [T][F]
  * ---------------------------------------------------------------------------------------------- */
 int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x_fp16, void* out_fp16, int T, b200_stream_t stream);
+/* The same GEMM with a bias b fp16 [N] added at the store (bias_mode B200_BIAS_ACC or B200_BIAS_OUT, as in b200_gemv_args_t);
+ * the codecs and shapes of b200_prefill_gemm_w4. */
+int b200_prefill_gemm_w4_bias(const b200_linear_t* lin, const void* x_fp16, const void* bias_fp16, int bias_mode,
+                              void* out_fp16, int T, b200_stream_t stream);
 /* Grouped MoE form of the same GEMM (Mixtral prompts, mixtral.py:266-294), one launch over a rank's local experts:
  * for each local expert i (global id e_first + i), for every slot s with slot_expert[s] == e_first + i:
  *   out[s][0:N] = x[s / src_div][0:K] . w_hat_i^T   (w_hat = fp16(fp16(q - z) * s16), fp32 accumulation, fp16 out)

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libb200decode.so")
 
 B200_PRO_NONE, B200_PRO_RMSNORM = 0, 1
 B200_EPI_F16, B200_EPI_F32, B200_EPI_QKV, B200_EPI_SILU = 0, 1, 2, 3
+B200_BIAS_NONE, B200_BIAS_ACC, B200_BIAS_OUT = 0, 1, 2
 
 
 class Linear(C.Structure):
@@ -35,6 +36,7 @@ class GemvArgs(C.Structure):
         ("ar_step", C.c_void_p), ("ar_out_id", C.c_int), ("ar_in_id", C.c_int), ("ar_period", C.c_int),
         ("ar_error", C.c_void_p),
         ("prefetch_const", C.c_void_p), ("prefetch_const_bytes", C.c_int),
+        ("bias", C.c_void_p), ("bias_mode", C.c_int),
     ]
 
 
@@ -118,6 +120,8 @@ SYMBOLS = {
     "b200_ipc_close": (C.c_int, [C.c_void_p]),
     "b200_ipc_free": (C.c_int, [C.c_void_p]),
     "b200_prefill_gemm_w4": (C.c_int, [C.POINTER(Linear), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "b200_prefill_gemm_w4_bias": (C.c_int, [C.POINTER(Linear), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                            C.c_void_p]),
     "b200_prefill_moe_gemm_w4": (C.c_int, [C.POINTER(Linear), C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),
     "b200_prefill_rmsnorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_int,

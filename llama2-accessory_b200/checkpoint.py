@@ -99,6 +99,71 @@ class SparseExpertView(Mapping):
         return blk.t().contiguous() if raw.endswith("w2") else blk.contiguous()
 
 
+def internlm_rope_perm(head_dim: int) -> torch.Tensor:
+    """Row order [0, hd/2, 1, hd/2 + 1, ...] of one head.  InternLM's RoPE (internlm.py:31-40) rotates the pair (i, i + hd/2)
+    and returns the pairs interleaved, so it equals LLaMA's RoPE (pairs 2i, 2i + 1, llama.py:59-77) applied to the q / k rows
+    taken in this order -- and the K cache then holds exactly what the reference's k_cache holds."""
+    h = head_dim // 2
+    return torch.stack([torch.arange(h), torch.arange(h) + h], dim=1).reshape(-1)
+
+
+_INTERNLM_LAYER = re.compile(r"^layers\.(\d+)\.(.+)$")
+_INTERNLM_NAMES = {"norm1.weight": "attention_norm.weight", "norm2.weight": "ffn_norm.weight",
+                   "mixer.out_proj.weight": "attention.wo.weight", "mixer.out_proj.bias": "attention.wo.bias",
+                   # internlm.py:181-196: w1 = gate, w2 = up ([F, D] although a RowParallelLinear), w3 = down [D, F]
+                   "mlp.w1.weight": "feed_forward.w1.weight", "mlp.w2.weight": "feed_forward.w3.weight",
+                   "mlp.w3.weight": "feed_forward.w2.weight"}
+
+
+class InternLMView(Mapping):
+    """An InternLM state dict (internlm.py) seen under the LLaMA names the engine loads: ``embedding`` / ``head`` / ``norm``
+    -> ``tok_embeddings`` / ``output`` / ``norm``; ``layers.{i}.norm1`` / ``norm2`` -> ``attention_norm`` / ``ffn_norm``; the fused
+    ``mixer.Wqkv`` [3D, D] (and its bias) -> ``attention.w{q,k,v}`` with the q and k rows of every head in internlm_rope_perm
+    order; ``mixer.out_proj`` -> ``attention.wo``; ``mlp.w1`` / ``w2`` / ``w3`` -> ``feed_forward.w1`` / ``w3`` / ``w2``.  Keys may carry
+    the ``llma.`` prefix.  Quantisation is per output row (groups along K), so it commutes with the row permutation: records
+    recovered from the viewed tensors are those of the reference's Wqkv, reordered."""
+
+    def __init__(self, sd: Mapping, n_heads: int):
+        self._sd, self._H = sd, n_heads
+        self._keys = OrderedDict()
+        for raw in sd:
+            k = raw[5:] if raw.startswith("llma.") else raw
+            top = {"embedding.weight": "tok_embeddings.weight", "head.weight": "output.weight"}
+            m = _INTERNLM_LAYER.match(k)
+            if k in top:
+                self._keys[top[k]] = (raw, None)
+            elif m and m.group(2) in ("mixer.Wqkv.weight", "mixer.Wqkv.bias"):
+                kind = m.group(2).rsplit(".", 1)[1]
+                for j, x in enumerate("qkv"):
+                    self._keys[f"layers.{m.group(1)}.attention.w{x}.{kind}"] = (raw, j)
+            elif m and m.group(2) in _INTERNLM_NAMES:
+                self._keys[f"layers.{m.group(1)}.{_INTERNLM_NAMES[m.group(2)]}"] = (raw, None)
+            else:
+                self._keys[k] = (raw, None)
+
+    def __len__(self):
+        return len(self._keys)
+
+    def __iter__(self):
+        return iter(self._keys)
+
+    def __contains__(self, key):
+        return key in self._keys
+
+    def __getitem__(self, key):
+        raw, j = self._keys[key]
+        w = self._sd[raw]
+        if j is None:
+            return w
+        D = w.shape[0] // 3
+        part = w[j * D:(j + 1) * D]
+        if j == 2:  # v: no RoPE, rows as stored
+            return part.contiguous()
+        hd = D // self._H
+        idx = (torch.arange(self._H)[:, None] * hd + internlm_rope_perm(hd)[None, :]).reshape(-1)
+        return part[idx].contiguous()
+
+
 def get_tensor_parallel_shards_file_name(format: str, mp_size: int) -> List[str]:
     """File name of every tensor-parallel shard of a checkpoint (tensor_parallel.py:171-197)."""
     if format == "meta_ori":
@@ -483,6 +548,10 @@ def _pl_to_dict(pl: Optional[PackedLinear]):
             "scales": None if pl.scales is None else pl.scales.cpu()}
 
 
+def _dev_or_none(t, device):
+    return None if t is None else t.to(device)
+
+
 def _pl_from_dict(d, device) -> Optional[PackedLinear]:
     if d is None:
         return None
@@ -507,7 +576,8 @@ def save_packed(engine, path: str) -> str:
         layers.append({"attn_norm": lw.attn_norm.cpu(), "ffn_norm": lw.ffn_norm.cpu(), "wqkv": _pl_to_dict(lw.wqkv),
                        "wo": _pl_to_dict(lw.wo), "w13": _pl_to_dict(lw.w13), "w2": _pl_to_dict(lw.w2),
                        "gate": None if lw.gate is None else lw.gate.cpu(),
-                       "e_w13": [_pl_to_dict(p) for p in lw.e_w13], "e_w2": [_pl_to_dict(p) for p in lw.e_w2]})
+                       "e_w13": [_pl_to_dict(p) for p in lw.e_w13], "e_w2": [_pl_to_dict(p) for p in lw.e_w2],
+                       "bqkv": None if lw.bqkv is None else lw.bqkv.cpu(), "bo": None if lw.bo is None else lw.bo.cpu()})
     blob = {"version": PACKED_FORMAT_VERSION, "config": asdict(c), "tok_emb": engine.tok_emb.cpu(),
             "final_norm": engine.final_norm.cpu(), "lm_head": _pl_to_dict(engine.lm_head), "layers": layers}
     fn = os.path.join(path, packed_shard_file_name(c.tp_rank, c.tp_world))
@@ -524,9 +594,10 @@ def load_packed(engine, path: str):
     if blob.get("version") != PACKED_FORMAT_VERSION:
         raise ValueError(f"packed shard version {blob.get('version')} != {PACKED_FORMAT_VERSION}")
     mine, theirs = asdict(c), blob["config"]
-    theirs = dict({"sparse_moe": False}, **theirs)  # shards written before mixtral_sparse existed: base Mixtral
+    # shards written before mixtral_sparse / internlm existed: base Mixtral, no attention biases
+    theirs = dict({"sparse_moe": False, "attn_bias": False}, **theirs)
     for k in ("kind", "dim", "n_layers", "n_heads", "n_kv_heads", "ffn_hidden", "vocab_size", "num_experts",
-              "experts_per_tok", "bits", "group_size", "tp_rank", "tp_world", "sparse_moe"):
+              "experts_per_tok", "bits", "group_size", "tp_rank", "tp_world", "sparse_moe", "attn_bias"):
         if mine[k] != theirs[k]:
             raise ValueError(f"packed shard was written for {k}={theirs[k]}, engine has {k}={mine[k]}")
     dev = engine.device
@@ -540,6 +611,7 @@ def load_packed(engine, path: str):
         lw.gate = None if d["gate"] is None else d["gate"].to(dev)
         lw.e_w13 = [_pl_from_dict(p, dev) for p in d["e_w13"]]
         lw.e_w2 = [_pl_from_dict(p, dev) for p in d["e_w2"]]
+        lw.bqkv, lw.bo = _dev_or_none(d.get("bqkv"), dev), _dev_or_none(d.get("bo"), dev)
     return engine
 
 
@@ -547,7 +619,8 @@ def load_packed(engine, path: str):
 # one call: checkpoint folder(s) -> engine
 # ---------------------------------------------------------------------------------------------------
 _KIND_OF_TYPE = {"llama": "llama", "llama_b200": "llama", "mixtral": "mixtral", "mixtral_b200": "mixtral",
-                 "mixtral_sparse": "mixtral_sparse", "mixtral_sparse_b200": "mixtral_sparse"}
+                 "mixtral_sparse": "mixtral_sparse", "mixtral_sparse_b200": "mixtral_sparse",
+                 "internlm": "internlm", "internlm_b200": "internlm"}
 
 
 def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, llama_type: Optional[str] = None,
@@ -571,13 +644,24 @@ def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, 
     if kind == "llama":  # defaults of llama.py:28-43
         for k, dflt in (("dim", 4096), ("n_layers", 32), ("n_heads", 32), ("multiple_of", 256), ("norm_eps", 1e-5)):
             args.setdefault(k, dflt)
+    elif kind == "internlm":  # defaults of internlm.py:45-64
+        for k, dflt in (("num_layers", 32), ("hidden_size", 4096), ("num_attention_heads", 32), ("mlp_ratio", 8 / 3),
+                        ("layer_norm_epsilon", 1e-5), ("norm_type", "rmsnorm"), ("use_swiglu", True), ("multiple_of", 256),
+                        ("rope_theta", 10000)):
+            args.setdefault(k, dflt)
     else:  # defaults of mixtral.py:33-54 (mixtral_sparse.py:47-68: the same)
         for k, dflt in (("dim", 4096), ("hidden_dim", 16384), ("n_layers", 32), ("n_heads", 32), ("norm_eps", 1e-5),
                         ("rope_theta", 1000000.0), ("moe", {"num_experts_per_tok": 2, "num_experts": 8})):
             args.setdefault(k, dflt)
     cfg = EngineConfig.from_model_args(kind, args, bits=bits, group_size=group_size, tp_rank=tp_rank, tp_world=tp_world)
-    eng = DecodeEngine(cfg, device, group=group)
     paths = [pretrained_path] if isinstance(pretrained_path, str) else list(pretrained_path)
+    if kind == "internlm":
+        for pth in paths:
+            if infer_checkpoint_format_and_mp_size(pth)[1] != 1:
+                raise ValueError(f"internlm: {pth} holds a tensor-parallel checkpoint; the reference module runs at TP = 1 "
+                                 "only (its Wqkv rows are not split per rank in q / k / v order), so only single-shard "
+                                 "folders are served")
+    eng = DecodeEngine(cfg, device, group=group)
     if len(paths) == 1:
         # streaming: every linear is merged from the memory-mapped shards, quantised (or recovered), sharded, packed and
         # dropped before the next one is touched -- peak host memory is one merged tensor, not the master model
@@ -586,6 +670,8 @@ def build_engine_from_pretrained(pretrained_path: Union[str, Sequence[str]], *, 
         sd = load_tensor_parallel_state_dict_list(paths, 0, 1)
     if kind == "mixtral_sparse":  # the stacked experts as per-expert linears, so that records are per expert
         sd = SparseExpertView(sd, cfg.num_experts)
+    elif kind == "internlm":  # the LLaMA names, q / k rows in RoPE order: records are keyed like a LLaMA model's
+        sd = InternLMView(sd, cfg.n_heads)
     recs = None
     if fake_quantised and bits != 16:
         recs = (LazyQuantRecords if len(paths) == 1 else recover_quant_records)(sd, bits, group_size)

@@ -31,8 +31,8 @@ namespace b200 {
 // 9..10 epilogue (cross-warp reduction, scales, fused epilogue, global stores).  Everything between the
 // roles is mbarrier-synchronised, so the dependent global loads of the epilogue never stall the MMA warps.
 // ------------------------------------------------------------------------------------------------
-template <int BITS, int NT, bool GROUPED>
-__global__ void __launch_bounds__(kThreads, 1) gemv_kernel(const __grid_constant__ GemvParams p) {
+template <int BITS, int NT, bool GROUPED, bool BIAS>
+__device__ __forceinline__ void gemv_body(const GemvParams& p, GemvBias bias) {
   using C = Codec<BITS>;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* ring = smem;
@@ -125,8 +125,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemv_kernel(const __grid_constant
   if (warp > kConsumerWarps) {
     // ---------------- epilogue warps ----------------
     int elt = 0;
-    epilogue_role<BITS, NT>(p, T, cols, nta, grouped, tid - (kConsumerWarps + 1) * 32, lane, red, red_full, red_empty,
-                            x_ready, xsum, elt, 0);
+    epilogue_role<BITS, NT, BIAS>(p, T, cols, nta, grouped, tid - (kConsumerWarps + 1) * 32, lane, red, red_full, red_empty,
+                            x_ready, xsum, elt, 0, bias);
     return;
   }
 
@@ -152,12 +152,23 @@ __global__ void __launch_bounds__(kThreads, 1) gemv_kernel(const __grid_constant
   }
 }
 
+template <int BITS, int NT, bool GROUPED>
+__global__ void __launch_bounds__(kThreads, 1) gemv_kernel(const __grid_constant__ GemvParams p) {
+  gemv_body<BITS, NT, GROUPED, false>(p, GemvBias{});
+}
+// the same kernel with the bias epilogue (B200_BIAS_ACC / _OUT): separate instances, so the bias-free ones are untouched
+template <int BITS, int NT, bool GROUPED>
+__global__ void __launch_bounds__(kThreads, 1) gemv_bias_kernel(const __grid_constant__ GemvBiasParams bp) {
+  gemv_body<BITS, NT, GROUPED, true>(bp.p, bp.bias);
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-template <int BITS, int NT, bool GROUPED>
-static int launch(const GemvParams& p, int grid, size_t smem, bool pdl, cudaStream_t st) {
-  auto kfn = gemv_kernel<BITS, NT, GROUPED>;
+template <int BITS, int NT, bool GROUPED, bool BIAS>
+static int launch(const GemvParams& p, GemvBias bias, int grid, size_t smem, bool pdl, cudaStream_t st) {
+  auto kfn = BIAS ? reinterpret_cast<const void*>(gemv_bias_kernel<BITS, NT, GROUPED>)
+                  : reinterpret_cast<const void*>(gemv_kernel<BITS, NT, GROUPED>);
   static size_t configured_dev[16] = {};  // cudaFuncSetAttribute is per device
   int dev = 0;
   cudaGetDevice(&dev);
@@ -181,7 +192,9 @@ static int launch(const GemvParams& p, int grid, size_t smem, bool pdl, cudaStre
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kfn, p);
+  cudaError_t e;
+  if constexpr (BIAS) e = cudaLaunchKernelEx(&cfg, gemv_bias_kernel<BITS, NT, GROUPED>, GemvBiasParams{p, bias});
+  else e = cudaLaunchKernelEx(&cfg, gemv_kernel<BITS, NT, GROUPED>, p);
   if (e != cudaSuccess) {
     set_error(std::string("gemv: launch: ") + cudaGetErrorString(e));
     return (int)e;
@@ -189,22 +202,28 @@ static int launch(const GemvParams& p, int grid, size_t smem, bool pdl, cudaStre
   return 0;
 }
 
-template <int BITS, bool GROUPED>
-static int launch_g(int NT, const GemvParams& p, int grid, size_t smem, bool pdl, cudaStream_t st) {
+template <int BITS, bool GROUPED, bool BIAS>
+static int launch_gb(int NT, const GemvParams& p, GemvBias bias, int grid, size_t smem, bool pdl, cudaStream_t st) {
   switch (NT) {
-    case 1: return launch<BITS, 1, GROUPED>(p, grid, smem, pdl, st);
-    case 2: return launch<BITS, 2, GROUPED>(p, grid, smem, pdl, st);
-    default: return launch<BITS, 4, GROUPED>(p, grid, smem, pdl, st);
+    case 1: return launch<BITS, 1, GROUPED, BIAS>(p, bias, grid, smem, pdl, st);
+    case 2: return launch<BITS, 2, GROUPED, BIAS>(p, bias, grid, smem, pdl, st);
+    default: return launch<BITS, 4, GROUPED, BIAS>(p, bias, grid, smem, pdl, st);
   }
 }
 
+template <int BITS, bool GROUPED>
+static int launch_g(int NT, const GemvParams& p, GemvBias bias, int grid, size_t smem, bool pdl, cudaStream_t st) {
+  return bias.b ? launch_gb<BITS, GROUPED, true>(NT, p, bias, grid, smem, pdl, st)
+                : launch_gb<BITS, GROUPED, false>(NT, p, bias, grid, smem, pdl, st);
+}
+
 template <int BITS>
-static int launch_nt(int NT, const GemvParams& p, int grid, size_t smem, bool pdl, cudaStream_t st) {
+static int launch_nt(int NT, const GemvParams& p, GemvBias bias, int grid, size_t smem, bool pdl, cudaStream_t st) {
   // grouped scales exist for the W4 and W2 codecs only (build_gemv_params rejects the rest)
   if constexpr (BITS == 4 || BITS == 2) {
-    if (p.G > 1) return launch_g<BITS, true>(NT, p, grid, smem, pdl, st);
+    if (p.G > 1) return launch_g<BITS, true>(NT, p, bias, grid, smem, pdl, st);
   }
-  return launch_g<BITS, false>(NT, p, grid, smem, pdl, st);
+  return launch_g<BITS, false>(NT, p, bias, grid, smem, pdl, st);
 }
 
 static size_t fixed_smem(int NT, int T, int n_chunk64, int x_stride, int stages) {
@@ -340,6 +359,28 @@ int b200::build_gemv_params(const b200_gemv_args_t* a, GemvParams* pp) {
     set_error("gemv: MoE slot indirection needs 1 <= n_slots == T <= 32 and a non-QKV epilogue");
     return B200_E_INVAL;
   }
+  if (a->bias_mode < B200_BIAS_NONE || a->bias_mode > B200_BIAS_OUT) {
+    set_error("gemv: bias_mode must be 0 (none), 1 (B200_BIAS_ACC) or 2 (B200_BIAS_OUT)");
+    return B200_E_INVAL;
+  }
+  if ((a->bias != nullptr) != (a->bias_mode != B200_BIAS_NONE)) {
+    set_error("gemv: a bias needs bias_mode 1 or 2, and bias_mode 1 or 2 needs a bias");
+    return B200_E_INVAL;
+  }
+  if (a->bias) {
+    if (p.epi != B200_EPI_F16 && p.epi != B200_EPI_QKV) {
+      set_error("gemv: a bias is supported with the fp16 and QKV epilogues only");
+      return B200_E_INVAL;
+    }
+    if (a->slot_expert) {
+      set_error("gemv: a bias cannot be combined with MoE slot indirection");
+      return B200_E_INVAL;
+    }
+    if (a->ar_world > 1) {
+      set_error("gemv: a bias cannot be combined with the fused all-reduce (it is added after the reduction)");
+      return B200_E_INVAL;
+    }
+  }
   p.x_stride = p.Kpad + kXPad;
   p.n_chunk64 = L.K / 64;
   if (a->ar_world > 1) {
@@ -459,12 +500,13 @@ extern "C" int b200_gemv(const b200_gemv_args_t* a, b200_stream_t stream) {
     p.next_tiles = a->prefetch_tiles;
     p.next_grid = std::min(std::max(a->prefetch_tiles, 1), sm_count());
     p.next_window = prefetch_window_bytes();
+    const GemvBias bias{static_cast<const __half*>(a->bias), a->bias_mode};
     int r;
     switch (bits) {
-      case 4: r = launch_nt<4>(NT, p, grid, smem, a->use_pdl != 0, st); break;
-      case 2: r = launch_nt<2>(NT, p, grid, smem, a->use_pdl != 0, st); break;
-      case 3: r = launch_nt<3>(NT, p, grid, smem, a->use_pdl != 0, st); break;
-      default: r = launch_nt<16>(NT, p, grid, smem, a->use_pdl != 0, st); break;
+      case 4: r = launch_nt<4>(NT, p, bias, grid, smem, a->use_pdl != 0, st); break;
+      case 2: r = launch_nt<2>(NT, p, bias, grid, smem, a->use_pdl != 0, st); break;
+      case 3: r = launch_nt<3>(NT, p, bias, grid, smem, a->use_pdl != 0, st); break;
+      default: r = launch_nt<16>(NT, p, bias, grid, smem, a->use_pdl != 0, st); break;
     }
     if (r) return r;
   }

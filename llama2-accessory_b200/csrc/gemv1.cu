@@ -29,8 +29,8 @@ namespace b200 {
 
 // ONE instance per scale layout: prologue and epilogue are run-time switches (gemv1_core.cuh, kDyn), so the four GEMV
 // launches of a layer execute the same instructions and find them cached.
-template <bool GROUPED>
-__global__ void __launch_bounds__(kThreads, 1) gemv1_kernel(const __grid_constant__ GemvParams p) {
+template <bool GROUPED, bool BIAS>
+__device__ __forceinline__ void gemv1_body(const GemvParams& p, GemvBias bias) {
   const int EPI = p.epi;
   extern __shared__ __align__(128) uint8_t smem[];
   G1Smem sm;
@@ -158,12 +158,22 @@ __global__ void __launch_bounds__(kThreads, 1) gemv1_kernel(const __grid_constan
   }
   if (warp > kConsumerWarps) {
     int lt = 0;
-    g1_epilogue_phase<kDyn, GROUPED, true>(p, sm, tid - (kConsumerWarps + 1) * 32, lane, cta, n_cta, lt, /*wait_dep=*/true);
+    g1_epilogue_phase<kDyn, GROUPED, true, BIAS>(p, sm, tid - (kConsumerWarps + 1) * 32, lane, cta, n_cta, lt, /*wait_dep=*/true, bias);
     return;
   }
   // griddepcontrol.wait happens inside the staging, after the constant loads (norm weight) have been issued
   G1State st;
   g1_mma_phase<kDyn, GROUPED, true>(p, sm, warp, lane, cta, n_cta, st, /*wait_dep=*/true, x_ready);
+}
+
+template <bool GROUPED>
+__global__ void __launch_bounds__(kThreads, 1) gemv1_kernel(const __grid_constant__ GemvParams p) {
+  gemv1_body<GROUPED, false>(p, GemvBias{});
+}
+// with the bias epilogue (B200_BIAS_ACC / _OUT): separate instances, so the bias-free ones are untouched
+template <bool GROUPED>
+__global__ void __launch_bounds__(kThreads, 1) gemv1_bias_kernel(const __grid_constant__ GemvBiasParams bp) {
+  gemv1_body<GROUPED, true>(bp.p, bp.bias);
 }
 
 static size_t g1_smem_bytes(int stages, int xq_stride, bool grouped, int KB) {
@@ -175,9 +185,9 @@ static size_t g1_smem_bytes(int stages, int xq_stride, bool grouped, int KB) {
   return b;
 }
 
-template <bool GROUPED>
-static int launch1g(const GemvParams& p, int xq_stride, int grid, size_t smem, bool pdl, cudaStream_t st) {
-  auto kfn = gemv1_kernel<GROUPED>;
+template <bool GROUPED, bool BIAS>
+static int launch1g(const GemvParams& p, GemvBias bias, int grid, size_t smem, bool pdl, cudaStream_t st) {
+  auto kfn = BIAS ? reinterpret_cast<const void*>(gemv1_bias_kernel<GROUPED>) : reinterpret_cast<const void*>(gemv1_kernel<GROUPED>);
   static size_t configured[16] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -201,7 +211,9 @@ static int launch1g(const GemvParams& p, int xq_stride, int grid, size_t smem, b
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kfn, p);
+  cudaError_t e;
+  if constexpr (BIAS) e = cudaLaunchKernelEx(&cfg, gemv1_bias_kernel<GROUPED>, GemvBiasParams{p, bias});
+  else e = cudaLaunchKernelEx(&cfg, gemv1_kernel<GROUPED>, p);
   if (e != cudaSuccess) {
     set_error(std::string("gemv1: launch: ") + cudaGetErrorString(e));
     return (int)e;
@@ -263,7 +275,9 @@ int gemv1_launch(const b200_gemv_args_t* a, GemvParams p, cudaStream_t st) {
   const int grid = std::min(p.n_tiles, sm_count());
   const bool pdl = a->use_pdl != 0;
   if (p.epi != B200_EPI_F16 && p.epi != B200_EPI_F32 && p.epi != B200_EPI_QKV && p.epi != B200_EPI_SILU) return B200_E_INVAL;
-  return p.G > 1 ? launch1g<true>(p, xq_stride, grid, smem, pdl, st) : launch1g<false>(p, xq_stride, grid, smem, pdl, st);
+  const GemvBias bias{static_cast<const __half*>(a->bias), a->bias_mode};
+  if (bias.b) return p.G > 1 ? launch1g<true, true>(p, bias, grid, smem, pdl, st) : launch1g<false, true>(p, bias, grid, smem, pdl, st);
+  return p.G > 1 ? launch1g<true, false>(p, bias, grid, smem, pdl, st) : launch1g<false, false>(p, bias, grid, smem, pdl, st);
 }
 
 }  // namespace b200

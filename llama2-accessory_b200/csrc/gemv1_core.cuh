@@ -489,9 +489,9 @@ __device__ __forceinline__ void g1_producer_phase(const GemvParams& p, const G1S
 // Thread etid owns rows r0 = etid/8 and r0+8 of a tile and plane column c = etid%8; the 8 lanes of a row group
 // exchange their columns with shuffles and then all hold the same y (only c == 0 stores).
 // ------------------------------------------------------------------------------------------------
-template <int EPI_T, bool GROUPED = false, bool ARED = false>
+template <int EPI_T, bool GROUPED = false, bool ARED = false, bool BIAS = false>
 __device__ __forceinline__ void g1_epilogue_phase(const GemvParams& p, const G1Smem& sm, int etid, int lane, int cta,
-                                                  int n_cta, int& lt_io, bool wait_dep = false) {
+                                                  int n_cta, int& lt_io, bool wait_dep = false, GemvBias bias = {}) {
   const int EPI = EPI_T == kDyn ? p.epi : EPI_T;
   const int tile_begin = (int)(((long long)p.n_tiles * cta) / n_cta);
   const int tile_end = (int)(((long long)p.n_tiles * (cta + 1)) / n_cta);
@@ -546,6 +546,8 @@ __device__ __forceinline__ void g1_epilogue_phase(const GemvParams& p, const G1S
         cs[hh] = staged ? rope_s[li * 16 + r0 + 8 * hh] : (rot ? p.rope[(size_t)ps * 64 + (d >> 1)] : make_float2(1.f, 0.f));
       }
     }
+    __half bias_r[2];
+    if (BIAS) bias_r[0] = bias.b[tile * 16 + r0], bias_r[1] = bias.b[tile * 16 + r0 + 8];
     mbar_wait(&sm.red_full[buf], (lt >> 1) & 1);
     const int* rbase = sm.red + (size_t)buf * kConsumerWarps * 128;
     float y[2];
@@ -615,7 +617,7 @@ __device__ __forceinline__ void g1_epilogue_phase(const GemvParams& p, const G1S
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int r = r0 + 8 * hh, row = tile * 16 + r;
-        const __half y16 = __float2half_rn(y[hh]);
+        const __half y16 = BIAS ? round_with_bias(y[hh], bias_r[hh], bias.mode) : __float2half_rn(y[hh]);
         if (EPI == B200_EPI_F16) {
           if (p.ll_out) {
             // fused all-reduce, push side: rows r0 / r0 ^ 1 sit in lanes 8 apart; the even one stores {half2, seq} to every rank

@@ -95,6 +95,23 @@ struct GemvParams {
   int dbg;  // experiment knob (B200_GEMV_DBG): 1 = skip the MMA math, 2 = skip the weight LDS too
 };
 
+// fp16 bias [N] of a linear and its rounding point (B200_BIAS_ACC / _OUT).  Kept out of GemvParams, which the persistent
+// kernels (mega1.cu, mega2.cu) hold in local memory: only the bias kernel instances take it, as a second member of their
+// parameter block (GemvBiasParams).
+struct GemvBias {
+  const __half* b;
+  int mode;
+};
+struct GemvBiasParams {
+  GemvParams p;
+  GemvBias bias;
+};
+
+// y (fp32 accumulator) + b rounded to fp16 at the bias's rounding point: fp16(y + b) or fp16(fp16(y) + b)
+__device__ __forceinline__ __half round_with_bias(float y, __half b, int mode) {
+  return mode == B200_BIAS_ACC ? __float2half_rn(__fadd_rn(y, __half2float(b))) : __hadd(__float2half_rn(y), b);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Codecs: one packed 512-byte k-block (uint4 per lane) -> HMMAs.  acc[nt][cls][4].
 // xr[nt] points at the lane's k-run of the staged x row for n-tile nt (block offset added here).
@@ -511,11 +528,11 @@ static __device__ void stage_x(const GemvParams& p, int T, const int* cols, __ha
 // Epilogue role (2 warps): wait for the 8 MMA-warp partials of a tile, reduce in fixed order, apply the
 // scales, round to fp16 and run the fused epilogue.  Shared by the TMA-ring and the direct-load kernels.
 // ------------------------------------------------------------------------------------------------
-template <int BITS, int NT>
+template <int BITS, int NT, bool BIAS = false>
 __device__ __forceinline__ void epilogue_role(const GemvParams& p, int T, const int* cols, int nta, bool grouped,
                                               int etid, int lane, const float* red, uint64_t* red_full,
                                               uint64_t* red_empty, uint64_t* x_ready, const float* xsum, int& lt,
-                                              uint32_t x_par) {
+                                              uint32_t x_par, GemvBias bias = {}) {
     pdl_wait();
     // positions of this thread's columns (QKV epilogue): loaded once, ahead of every dependent rope load
     int ps_col[NT];
@@ -579,6 +596,8 @@ __device__ __forceinline__ void epilogue_role(const GemvParams& p, int T, const 
                                          : (rot ? p.rope[(size_t)ps_col[nt] * 64 + (d >> 1)] : make_float2(1.f, 0.f));
         }
       }
+      __half bias_r[2];
+      if (BIAS) bias_r[0] = bias.b[tile * 16 + r0], bias_r[1] = bias.b[tile * 16 + r0 + 8];
       mbar_wait(&red_full[buf], (lt >> 1) & 1);
       const float* rbase = red + (size_t)buf * kConsumerWarps * (NT * 128);
 #pragma unroll
@@ -612,7 +631,7 @@ __device__ __forceinline__ void epilogue_role(const GemvParams& p, int T, const 
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const int r = r0 + 8 * hh, row = tile * 16 + r;
-            const __half y16 = __float2half_rn(y[hh]);
+            const __half y16 = BIAS ? round_with_bias(y[hh], bias_r[hh], bias.mode) : __float2half_rn(y[hh]);
             if (p.epi == B200_EPI_F16) {
               if (NT == 1 && p.ll_out) {
                 // fused all-reduce, push side (T == 1, so NT == 1 only: the larger instances carry no push code; as

@@ -74,6 +74,8 @@ struct Params {
   const __half* x;       // [T][K]
   __half* out;           // [T][N]
   int N, K, KB, T, T_pad;  // KB: pipeline stages over K; T_pad = NC * 32 >= T, <= 256
+  const __half* bias;      // [N] fp16, read only by the kBias instances (b200_prefill_gemm_w4_bias)
+  int bias_mode;           // B200_BIAS_ACC: fp16(acc + b); B200_BIAS_OUT: fp16(fp16(acc) + b)
 };
 
 // K-major, SWIZZLE_128B canonical layout of a [rows x 64] fp16 tile: 8-row groups of 1024 B, 16-byte chunk c of row r
@@ -150,7 +152,7 @@ __device__ __forceinline__ uint32_t deq_pair_w3(uint32_t w, __half2 zoff, __half
 
 // One CTA of the GEMM: 128 output rows x p.T (<= NC * 32) tokens.  kRouted (the grouped MoE GEMM): token t of the CTA is
 // slot rows[t] (shared memory); its activations are row rows[t] / src_div of p.x and its outputs row rows[t] of p.out.
-template <Codec C, int NC, bool kRouted>
+template <Codec C, int NC, bool kRouted, bool kBias = false>
 __device__ __forceinline__ void gemm_cta(const Params& p, uint8_t* smem_raw, const int* rows, int src_div) {
   using S = Stage<C>;
   constexpr int kBBytes = S::kBBytes, kPackedBytes = S::kPackedBytes;
@@ -252,8 +254,17 @@ __device__ __forceinline__ void gemm_cta(const Params& p, uint8_t* smem_raw, con
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int t = c * 32 + i * 8 + 2 * t4 + e, row = row0 + warp * 16 + g + 8 * h;
-            if (t < p.T && row < p.N)
-              p.out[(size_t)(kRouted ? rows[t] : t) * p.N + row] = __float2half_rn(acc[c][4 * i + 2 * h + e]);
+            if (t < p.T && row < p.N) {
+              const float y = acc[c][4 * i + 2 * h + e];
+              __half o;
+              if constexpr (kBias) {
+                const __half b = p.bias[row];
+                o = p.bias_mode == B200_BIAS_ACC ? __float2half_rn(__fadd_rn(y, __half2float(b))) : __hadd(__float2half_rn(y), b);
+              } else {
+                o = __float2half_rn(y);
+              }
+              p.out[(size_t)(kRouted ? rows[t] : t) * p.N + row] = o;
+            }
           }
   } else {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
@@ -350,6 +361,12 @@ template <int NC>
 __global__ void __launch_bounds__(kThreads, 1) prefill_gemm_f16_kernel(const __grid_constant__ Params p) {
   extern __shared__ uint8_t smem_raw[];
   gemm_cta<Codec::F16, NC, false>(p, smem_raw, nullptr, 1);
+}
+// b200_prefill_gemm_w4_bias: the same CTA with the bias added at the store (separate instances; the ones above are untouched)
+template <Codec C, int NC>
+__global__ void __launch_bounds__(kThreads, 1) prefill_gemm_bias_kernel(const __grid_constant__ Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  gemm_cta<C, NC, false, true>(p, smem_raw, nullptr, 1);
 }
 
 // ---- grouped MoE GEMM: the same CTA over the slots routed to one expert -------------------------------------------------
@@ -497,19 +514,21 @@ namespace b200 {
 namespace prefill {
 
 using GemmKernel = void (*)(Params);
-template <Codec C, int NC>
+template <Codec C, int NC, bool kBias>
 constexpr GemmKernel gemm_kernel() {
-  if constexpr (C == Codec::W4) return prefill_gemm_w4_kernel<NC>;
+  if constexpr (kBias) return prefill_gemm_bias_kernel<C, NC>;
+  else if constexpr (C == Codec::W4) return prefill_gemm_w4_kernel<NC>;
   else if constexpr (C == Codec::W3) return prefill_gemm_w3_kernel<NC>;
   else return prefill_gemm_f16_kernel<NC>;
 }
 
-template <Codec C>
-int launch_gemm(const b200_linear_t* lin, const void* x, void* out, int T, cudaStream_t stream) {
+template <Codec C, bool kBias = false>
+int launch_gemm(const b200_linear_t* lin, const void* x, void* out, int T, cudaStream_t stream, const void* bias = nullptr,
+                int bias_mode = 0) {
   using S = Stage<C>;
-  static const GemmKernel kernels[kMaxT / kNChunk] = {gemm_kernel<C, 1>(), gemm_kernel<C, 2>(), gemm_kernel<C, 3>(),
-                                                      gemm_kernel<C, 4>(), gemm_kernel<C, 5>(), gemm_kernel<C, 6>(),
-                                                      gemm_kernel<C, 7>(), gemm_kernel<C, 8>()};
+  static const GemmKernel kernels[kMaxT / kNChunk] = {
+      gemm_kernel<C, 1, kBias>(), gemm_kernel<C, 2, kBias>(), gemm_kernel<C, 3, kBias>(), gemm_kernel<C, 4, kBias>(),
+      gemm_kernel<C, 5, kBias>(), gemm_kernel<C, 6, kBias>(), gemm_kernel<C, 7, kBias>(), gemm_kernel<C, 8, kBias>()};
   static bool configured[16] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -532,6 +551,8 @@ int launch_gemm(const b200_linear_t* lin, const void* x, void* out, int T, cudaS
     p.x = static_cast<const __half*>(x) + (size_t)t0 * lin->K;
     p.out = static_cast<__half*>(out) + (size_t)t0 * lin->N;
     p.N = lin->N, p.K = lin->K, p.KB = (lin->K + S::kK - 1) / S::kK, p.T = std::min(kMaxT, T - t0);
+    p.bias = static_cast<const __half*>(bias);
+    p.bias_mode = bias_mode;
     const int nc = (p.T + kNChunk - 1) / kNChunk;
     p.T_pad = nc * kNChunk;
     kernels[nc - 1]<<<lin->N / BM, kThreads, S::kSmemBytes, stream>>>(p);
@@ -547,7 +568,7 @@ int launch_gemm(const b200_linear_t* lin, const void* x, void* out, int T, cudaS
 }  // namespace prefill
 }  // namespace b200
 
-extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, void* out, int T, b200_stream_t stream) {
+static int check_prefill_linear(const b200_linear_t* lin, const void* x, void* out, int T) {
   using namespace b200::prefill;
   if (!lin || !x || !out || T < 1) return B200_E_INVAL;
   const int bits = lin->bits;
@@ -558,10 +579,34 @@ extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, voi
               "required");
     return B200_E_UNSUPPORTED;
   }
+  return 0;
+}
+
+extern "C" int b200_prefill_gemm_w4(const b200_linear_t* lin, const void* x, void* out, int T, b200_stream_t stream) {
+  using namespace b200::prefill;
+  const int rc = check_prefill_linear(lin, x, out, T);
+  if (rc) return rc;
+  const int bits = lin->bits;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (bits == 4) return launch_gemm<Codec::W4>(lin, x, out, T, st);
   if (bits == 3) return launch_gemm<Codec::W3>(lin, x, out, T, st);
   return launch_gemm<Codec::F16>(lin, x, out, T, st);
+}
+
+extern "C" int b200_prefill_gemm_w4_bias(const b200_linear_t* lin, const void* x, const void* bias, int bias_mode, void* out,
+                                         int T, b200_stream_t stream) {
+  using namespace b200::prefill;
+  if (!bias || (bias_mode != B200_BIAS_ACC && bias_mode != B200_BIAS_OUT)) {
+    set_error("prefill_gemm_w4_bias: needs a bias and bias_mode 1 (B200_BIAS_ACC) or 2 (B200_BIAS_OUT)");
+    return B200_E_INVAL;
+  }
+  const int rc = check_prefill_linear(lin, x, out, T);
+  if (rc) return rc;
+  const int bits = lin->bits;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (bits == 4) return launch_gemm<Codec::W4, true>(lin, x, out, T, st, bias, bias_mode);
+  if (bits == 3) return launch_gemm<Codec::W3, true>(lin, x, out, T, st, bias, bias_mode);
+  return launch_gemm<Codec::F16, true>(lin, x, out, T, st, bias, bias_mode);
 }
 
 extern "C" int b200_prefill_moe_gemm_w4(const b200_linear_t* experts, int e_first, int e_count, const int32_t* slot_expert,

@@ -74,6 +74,8 @@ class EngineConfig:
     tp_world: int = 1
     # mixtral_sparse: every rank holds 1/TP of every expert (ffn_hidden / TP rows), fp32 router scores
     sparse_moe: bool = False
+    # internlm: fp16 biases on the fused QKV projection (added before RoPE, fp16(acc + b)) and on wo (fp16(fp16(acc) + b))
+    attn_bias: bool = False
 
     @property
     def head_dim(self):
@@ -85,7 +87,10 @@ class EngineConfig:
 
     @classmethod
     def from_model_args(cls, kind, a: dict, **kw):
-        """kind: 'llama' | 'mixtral' | 'mixtral_sparse' (served as kind 'mixtral' with sparse_moe = True)."""
+        """kind: 'llama' | 'mixtral' | 'mixtral_sparse' (served as kind 'mixtral' with sparse_moe = True) | 'internlm'
+        (internlm.py's ModelArgs, served as kind 'llama' with attn_bias = True)."""
+        if kind == "internlm":
+            return cls._from_internlm_args(a, **kw)
         if kind == "mixtral_sparse":
             kind, kw = "mixtral", dict(kw, sparse_moe=True)
         if kind == "llama":
@@ -102,6 +107,26 @@ class EngineConfig:
                    max_seq_len=a.get("max_seq_len", 2048), max_batch_size=a.get("max_batch_size", 32),
                    num_experts=ne, experts_per_tok=nk, **kw)
 
+    @classmethod
+    def _from_internlm_args(cls, a: dict, **kw):
+        """internlm.py ModelArgs: an MHA LLaMA block with Wqkv / out_proj biases.  The reference module itself only runs at
+        TP = 1 (its mlp.w2 is a RowParallelLinear fed the full hidden state, and a rank's contiguous Wqkv rows would mix q, k
+        and v in its `(three h d)` split), so tensor parallelism is refused."""
+        if a.get("norm_type", "rmsnorm") != "rmsnorm":
+            raise ValueError(f"internlm: norm_type {a.get('norm_type')!r} is not served (the decode kernels fuse RMSNorm only)")
+        if not a.get("use_swiglu", True):
+            raise ValueError("internlm: use_swiglu = False is not served (the FFN kernels compute SwiGLU)")
+        if kw.get("tp_world", 1) > 1:
+            raise ValueError("internlm: tensor parallelism is not supported -- the reference module runs at TP = 1 only "
+                             "(mlp.w2 is a RowParallelLinear fed the full hidden state, and the (three h d) split of a rank's "
+                             "Wqkv rows would mix q, k and v)")
+        D, mult = a["hidden_size"], a.get("multiple_of", 256)
+        ffn = mult * ((int(D * a.get("mlp_ratio", 8 / 3)) + mult - 1) // mult)  # internlm.py:190-211
+        return cls(kind="llama", dim=D, n_layers=a["num_layers"], n_heads=a["num_attention_heads"], n_kv_heads=None,
+                   ffn_hidden=ffn, vocab_size=a["vocab_size"], norm_eps=a.get("layer_norm_epsilon", 1e-5),
+                   rope_theta=a.get("rope_theta", 10000.0), rope_scaling=a.get("rope_scaling"),
+                   max_seq_len=a.get("max_seq_len", 2048), max_batch_size=a.get("max_batch_size", 32), attn_bias=True, **kw)
+
 
 @dataclass
 class LayerWeights:
@@ -114,6 +139,8 @@ class LayerWeights:
     gate: torch.Tensor = None      # mixtral: fp16 [E, D]
     e_w13: List[PackedLinear] = field(default_factory=list)
     e_w2: List[PackedLinear] = field(default_factory=list)
+    bqkv: torch.Tensor = None      # attn_bias: fp16 [(Hq + 2 Hkv) * 128], [bq; bk; bv] like the rows of wqkv
+    bo: torch.Tensor = None        # attn_bias: fp16 [dim]
 
 
 def rope_table(head_dim, end, theta, scaling):
@@ -133,6 +160,16 @@ def _interleave_w13(a, b):
     assert n % 8 == 0 and a.shape == b.shape
     return torch.stack([a.reshape(n // 8, 8, *a.shape[1:]), b.reshape(n // 8, 8, *b.shape[1:])], dim=1).reshape(
         2 * n, *a.shape[1:])
+
+
+def _qkv_bias(lw):
+    """internlm's Wqkv bias: F.linear(x, W, b), one fp16 rounding of acc + b (internlm.py:75-80)."""
+    return {} if lw.bqkv is None else dict(bias=lw.bqkv, bias_mode=ops.B200_BIAS_ACC)
+
+
+def _wo_bias(lw):
+    """internlm's out_proj bias: RowParallelLinear adds it to the fp16 output after the all-reduce (internlm.py:83-89)."""
+    return {} if lw.bo is None else dict(bias=lw.bo, bias_mode=ops.B200_BIAS_OUT)
 
 
 def check_kernel_limits(cfg: "EngineConfig"):
@@ -167,6 +204,8 @@ class DecodeEngine:
             raise ValueError("the decode kernels are specialised for head_dim = 128")
         if cfg.n_heads % cfg.tp_world or cfg.kv_heads % cfg.tp_world:
             raise ValueError("n_heads and n_kv_heads must be divisible by the tensor-parallel size")
+        if cfg.attn_bias and (cfg.kind != "llama" or cfg.tp_world > 1):
+            raise ValueError("attention biases (internlm) are served for dense models at tp_world = 1 only")
         check_kernel_limits(cfg)
         self.cfg = cfg
         self.device = torch.device(device)
@@ -348,6 +387,10 @@ class DecodeEngine:
             from .checkpoint import SparseExpertView
             if not isinstance(sd, SparseExpertView):
                 sd = SparseExpertView(sd, c.num_experts)
+        if c.attn_bias:  # an InternLM state dict is read under the LLaMA names (checkpoint.InternLMView)
+            from .checkpoint import InternLMView
+            if not isinstance(sd, InternLMView) and "embedding.weight" in sd:
+                sd = InternLMView(sd, c.n_heads)
         bits, gs, dev = c.bits, c.group_size, self.device
         emb = sd["tok_embeddings.weight"].to(torch.float16).to(dev).contiguous()
         if _sharded and c.tp_world > 1:  # [vocab, D/TP] shards -> full replicated table
@@ -367,6 +410,10 @@ class DecodeEngine:
                                         cat=[p + "attention.wq.weight", p + "attention.wk.weight",
                                              p + "attention.wv.weight"])
             lw.wo = self._make_linear(p + "attention.wo.weight", sd, quant_records, bits, gs, row)
+            if c.attn_bias:
+                b = [sd[p + f"attention.w{x}.bias"].to(torch.float16) for x in "qkv"]
+                lw.bqkv = torch.cat(b).to(dev).contiguous()
+                lw.bo = sd[p + "attention.wo.bias"].to(torch.float16).to(dev).contiguous()
             if c.kind == "llama":
                 fpad = self.F - self.F_raw
                 lw.w13 = self._make_linear(p + "feed_forward.w1.weight", sd, quant_records, bits, gs, col,
@@ -399,6 +446,9 @@ class DecodeEngine:
             lw.wqkv = random_packed(c.bits, (self.Hq + 2 * self.Hkv) * 128, D, c.group_size, dev, s)
             lw.wo = random_packed(c.bits, D, self.Hq * 128, c.group_size, dev, s + 1)
             s += 2
+            if c.attn_bias:
+                lw.bqkv = ((torch.rand(lw.wqkv.N, device=dev, generator=g) * 2 - 1) * 0.5).half()
+                lw.bo = ((torch.rand(D, device=dev, generator=g) * 2 - 1) * 0.5).half()
             if c.kind == "llama":
                 lw.w13 = random_packed(c.bits, 2 * self.F, D, c.group_size, dev, s)
                 lw.w2 = random_packed(c.bits, D, self.F, c.group_size, dev, s + 1)
@@ -509,7 +559,7 @@ class DecodeEngine:
             nxt = self.layers[i + 1].wqkv if i + 1 < len(self.layers) else self.lm_head
             ar_in = self._ar_args(in_buf=st["in_f"], in_id=2 * (i - 1) + 1) if (fused and delta is not None) else None
             ops.gemv(lw.wqkv, T, resid=self.h[cur], delta=delta, h_out=h_out, gamma=lw.attn_norm, eps=c.norm_eps,
-                     epilogue=ops.B200_EPI_QKV, out=self.q, use_pdl=pdl, ar=ar_in,
+                     epilogue=ops.B200_EPI_QKV, out=self.q, use_pdl=pdl, ar=ar_in, **_qkv_bias(lw),
                      qkv=dict(n_q_rows=self.Hq * 128, n_kv_rows=self.Hkv * 128, rope=self.rope, pos=self.pos,
                               tokens_per_seq=tokens_per_seq, kcache=kc, vtcache=vt, cache_seq=self.cache_seq,
                               prefetch_kv=bool(PF)))
@@ -522,7 +572,7 @@ class DecodeEngine:
                 nxt_norm = self.layers[i + 1].attn_norm if i + 1 < len(self.layers) else self.final_norm
                 ops.gemv(lw.wo, T, xin=self.attn, epilogue=ops.B200_EPI_F16, out=self.o, use_pdl=pdl,
                          prefetch=head(lw.w13), ar=self._ar_args(out_peers=st["peers_o"], out_id=2 * i) if fused else None,
-                         prefetch_const=lw.ffn_norm if PF else None)
+                         prefetch_const=lw.ffn_norm if PF else None, **_wo_bias(lw))
                 if not fused:
                     self._allreduce(self.o, T)
                 ops.gemv(lw.w13, T, resid=self.h[cur], delta=self.o, h_out=self.h[1 - cur], gamma=lw.ffn_norm,
@@ -572,7 +622,7 @@ class DecodeEngine:
 
     def mega_supported(self, T, row0=0, want_logits=True, last_rows=None):
         c = self.cfg
-        return (self.use_mega and c.kind == "llama" and T == 1 and c.bits == 4 and not c.group_size
+        return (self.use_mega and c.kind == "llama" and T == 1 and c.bits == 4 and not c.group_size and not c.attn_bias
                 and want_logits and last_rows is None and row0 == 0 and c.dim <= 8192 and self.F <= 16384
                 and self.Hq // self.Hkv <= 8 and c.n_layers <= 96 and self.lm_head is not None and self.lm_head.bits == 16
                 and not self.shard_only and c.tp_world <= 8)
@@ -722,7 +772,7 @@ class DecodeEngine:
                                 b["x"], T, c.dim)
             if delta is not None:
                 cur = 1 - cur
-            ops.prefill_gemm_w4(lw.wqkv, b["x"], b["qkv"], T)
+            ops.prefill_gemm_w4(lw.wqkv, b["x"], b["qkv"], T, **_qkv_bias(lw))
             ops.prefill_rope_kv(b["qkv"], b["q"], kc, vt, self.rope, b["pos"], T, nq, nkv, tokens_per_seq, self.cache_seq)
             for t0 in range(0, T, T_MAX):  # sub-chunks stay inside one sequence when tokens_per_seq % 32 == 0 or nb == 1
                 tn = min(T_MAX, T - t0)
@@ -735,7 +785,7 @@ class DecodeEngine:
                 ops.attn_decode(b["q"][t0:], kc[rb:], vt[rb:], b["pos"][t0:], b["attn"][t0:], T=tn, Hq=self.Hq, Hkv=self.Hkv,
                                 cache_seq=self.cache_seq, tokens_per_seq=tps, max_kv_len=max_kv_len, ws=self.ws,
                                 counters=self.counters, n_split=n_split, use_pdl=False)
-            ops.prefill_gemm_w4(lw.wo, b["attn"], b["o"], T)
+            ops.prefill_gemm_w4(lw.wo, b["attn"], b["o"], T, **_wo_bias(lw))
             self._allreduce(b["o"], T)
             if c.kind == "llama":
                 ops.prefill_rmsnorm(b["h"][cur], b["o"], b["h"][1 - cur], lw.ffn_norm, c.norm_eps, b["x"], T, c.dim)
@@ -952,6 +1002,9 @@ class DecodeEngine:
                     w += pl.nbytes
             for pl in lw.e_w13 + lw.e_w2:
                 w += pl.nbytes
+            for b in (lw.bqkv, lw.bo):
+                if b is not None:
+                    w += b.numel() * b.element_size()
         head = self.lm_head.nbytes
         kv = 2 * c.n_layers * ctx * self.Hkv * 128 * 2 * bsz
         return {"weights": w, "lm_head": head, "kv": kv, "total": w + head + kv}

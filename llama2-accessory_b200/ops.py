@@ -9,8 +9,8 @@ import ctypes as C
 import torch
 
 from . import _cabi
-from ._cabi import (B200_EPI_F16, B200_EPI_F32, B200_EPI_QKV, B200_EPI_SILU, B200_PRO_NONE,  # noqa: F401
-                    B200_PRO_RMSNORM)
+from ._cabi import (B200_BIAS_ACC, B200_BIAS_NONE, B200_BIAS_OUT, B200_EPI_F16, B200_EPI_F32, B200_EPI_QKV,  # noqa: F401
+                    B200_EPI_SILU, B200_PRO_NONE, B200_PRO_RMSNORM)
 from .quant import PackedLinear
 
 launch_count = 0  # kernels launched through this module (bench.py reports it as gpu_launches)
@@ -31,11 +31,13 @@ def _f16(t, name):
 
 def gemv(lin: PackedLinear, T: int, *, out, epilogue=B200_EPI_F16, xin=None, resid=None, delta=None, h_out=None,
          gamma=None, eps=1e-5, qkv=None, moe=None, use_pdl=False, ring_bytes=0, prefetch=None, ar=None,
-         prefetch_const=None):
-    """Fused [residual + RMSNorm] -> W-bit GEMV -> epilogue.  See include/b200_decode.h b200_gemv."""
+         prefetch_const=None, bias=None, bias_mode=B200_BIAS_NONE):
+    """Fused [residual + RMSNorm] -> W-bit GEMV -> epilogue.  See include/b200_decode.h b200_gemv.
+    bias: optional fp16 [N] added at bias_mode's rounding point (B200_BIAS_ACC / B200_BIAS_OUT)."""
     global launch_count
     a = gemv_args(lin, T, out=out, epilogue=epilogue, xin=xin, resid=resid, delta=delta, h_out=h_out, gamma=gamma,
-                  eps=eps, qkv=qkv, moe=moe, use_pdl=use_pdl, ring_bytes=ring_bytes, prefetch=prefetch)
+                  eps=eps, qkv=qkv, moe=moe, use_pdl=use_pdl, ring_bytes=ring_bytes, prefetch=prefetch, bias=bias,
+                  bias_mode=bias_mode)
     if prefetch_const is not None:  # a later launch's norm weight -> L2 now
         a.prefetch_const, a.prefetch_const_bytes = prefetch_const.data_ptr(), prefetch_const.numel() * prefetch_const.element_size()
     if ar is not None:  # fused tensor-parallel all-reduce (engine.DecodeEngine._ar): dict(world, rank, step, period, err, ...)
@@ -50,9 +52,12 @@ def gemv(lin: PackedLinear, T: int, *, out, epilogue=B200_EPI_F16, xin=None, res
 
 
 def gemv_args(lin: PackedLinear, T: int, *, out, epilogue=B200_EPI_F16, xin=None, resid=None, delta=None, h_out=None,
-              gamma=None, eps=1e-5, qkv=None, moe=None, use_pdl=False, ring_bytes=0, prefetch=None):
-    for t, n in ((xin, "xin"), (resid, "resid"), (delta, "delta"), (h_out, "h_out"), (gamma, "gamma")):
+              gamma=None, eps=1e-5, qkv=None, moe=None, use_pdl=False, ring_bytes=0, prefetch=None, bias=None,
+              bias_mode=B200_BIAS_NONE):
+    for t, n in ((xin, "xin"), (resid, "resid"), (delta, "delta"), (h_out, "h_out"), (gamma, "gamma"), (bias, "bias")):
         _f16(t, n)
+    if bias is not None and bias.numel() != lin.N:
+        raise ValueError(f"bias has {bias.numel()} elements, the linear has {lin.N} output rows")
     a = _cabi.GemvArgs()
     a.lin = lin.c_struct()
     a.T = T
@@ -75,6 +80,7 @@ def gemv_args(lin: PackedLinear, T: int, *, out, epilogue=B200_EPI_F16, xin=None
     if prefetch is not None:  # (tensor, nbytes[, tiles]): head of the next kernel's HBM stream -> L2
         a.prefetch_next, a.prefetch_bytes = prefetch[0].data_ptr(), int(prefetch[1])
         a.prefetch_tiles = int(prefetch[2]) if len(prefetch) > 2 else 0
+    a.bias, a.bias_mode = _p(bias), bias_mode
     return a
 
 
@@ -122,15 +128,21 @@ def _anchor(t, name):
     return t
 
 
-def prefill_gemm_w4(lin: PackedLinear, x, out, T):
+def prefill_gemm_w4(lin: PackedLinear, x, out, T, bias=None, bias_mode=B200_BIAS_ACC):
     """out[T, N] = x[T, K] . w_hat^T on the tensor cores (wgmma): per-channel W4 or W3, or fp16 weights (w_hat = w);
-    N % 128 == 0, K % 64 == 0 (W3: K % 16 == 0)."""
+    N % 128 == 0, K % 64 == 0 (W3: K % 16 == 0).  bias: optional fp16 [N] added at bias_mode's rounding point
+    (b200_prefill_gemm_w4_bias)."""
     global launch_count
     on = _anchor(x, "x")
     _dev(x, "x", torch.float16, T * lin.K, on)
     _dev(out, "out", torch.float16, T * lin.N, on)
     ls = lin.c_struct()
-    _cabi.check(_cabi.lib().b200_prefill_gemm_w4(C.byref(ls), _p(x), _p(out), T, _stream()), "b200_prefill_gemm_w4")
+    if bias is None:
+        _cabi.check(_cabi.lib().b200_prefill_gemm_w4(C.byref(ls), _p(x), _p(out), T, _stream()), "b200_prefill_gemm_w4")
+    else:
+        _dev(bias, "bias", torch.float16, lin.N, on)
+        _cabi.check(_cabi.lib().b200_prefill_gemm_w4_bias(C.byref(ls), _p(x), _p(bias), bias_mode, _p(out), T, _stream()),
+                    "b200_prefill_gemm_w4_bias")
     launch_count += (T + 255) // 256
 
 
