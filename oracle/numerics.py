@@ -83,18 +83,12 @@ def tuned(name, value):
 
 # ------------------------------------------------------------------------------------------- moe_route model --------
 def kernel_scores(logits16):
-    """fp16 [T, E] gate logits -> fp32 [T, E] fp16-valued scores: fp32 softmax with the experts summed in index order."""
-    lg = logits16.float().cpu().numpy()
-    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
-    den = np.zeros(lg.shape[0], dtype=np.float32)
-    for e in range(lg.shape[1]):                       # sequential fp32 sum over experts, as thread 0 does
-        den = (den + ex[:, e]).astype(np.float32)
-    return (ex / den[:, None]).astype(np.float32).astype(np.float16).astype(np.float32)
+    """fp16 [T, E] gate logits -> fp32 [T, E] fp16-valued scores: the fp32 softmax of kernel_scores_f32 rounded to fp16."""
+    return kernel_scores_f32(logits16).astype(np.float16).astype(np.float32)
 
 
-def kernel_route(logits16, k):
-    """logits16: fp16 [T, E] -> (idx int64 [T, k], weight fp16 [T, k]) following moe.cu line by line (numpy fp32)."""
-    sc = kernel_scores(logits16)
+def _route_top_k(sc, k):
+    """Top-k of fp32 scores [T, E] in rank order, ties to the lower index (the kernel's strict `>` scan from e = 0)."""
     T, E = sc.shape
     idx = np.zeros((T, k), dtype=np.int64)
     val = np.zeros((T, k), dtype=np.float32)
@@ -104,12 +98,93 @@ def kernel_route(logits16, k):
         b = masked.argmax(-1)                          # first maximum = lowest index on ties
         idx[:, j], val[:, j] = b, masked[np.arange(T), b]
         used[np.arange(T), b] = True
-    s = np.zeros(T, dtype=np.float32)
+    return idx, val
+
+
+def kernel_route(logits16, k):
+    """logits16: fp16 [T, E] -> (idx int64 [T, k], weight fp16 [T, k]) following moe.cu line by line (numpy fp32)."""
+    idx, val = _route_top_k(kernel_scores(logits16), k)
+    s = np.zeros(idx.shape[0], dtype=np.float32)
     for j in range(k):
         s = (s + val[:, j]).astype(np.float32)
     s16 = s.astype(np.float16).astype(np.float32)
     w = (val / s16[:, None]).astype(np.float32).astype(np.float16)
     return torch.from_numpy(idx), torch.from_numpy(w)
+
+
+def kernel_scores_f32(logits16):
+    """fp16 [T, E] gate logits -> fp32 [T, E] unrounded scores of moe_route_kernel<true>: expf(l - max) / den, den the
+    fp32 sum of the exponentials over the experts in index order (thread 0's loop)."""
+    lg = logits16.float().cpu().numpy()
+    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
+    den = np.zeros(lg.shape[0], dtype=np.float32)
+    for e in range(lg.shape[1]):
+        den = (den + ex[:, e]).astype(np.float32)
+    return (ex / den[:, None]).astype(np.float32)
+
+
+def kernel_route_f32(logits16, k):
+    """logits16: fp16 [T, E] -> (idx int64 [T, k], weight fp16 [T, k]) following moe_route_kernel<true> line by line
+    (numpy fp32): top-k on the unrounded fp32 scores (ties to the lower index), the fp32 sum of the chosen scores in rank
+    order, weight = fp16(score / sum) rounded once (mixtral_sparse.py:417-428)."""
+    idx, val = _route_top_k(kernel_scores_f32(logits16), k)
+    s = np.zeros(idx.shape[0], dtype=np.float32)
+    for j in range(k):
+        s = (s + val[:, j]).astype(np.float32)
+    w = (val / s[:, None]).astype(np.float32).astype(np.float16)
+    return torch.from_numpy(idx), torch.from_numpy(w)
+
+
+def route_f32(logits16, k):
+    """mixtral_sparse.py:417-428 stated in torch on fp16 logits [T, E]: fp32 softmax, top-k on the fp32 scores (ties:
+    lower index), fp32 renormalisation, one cast to fp16.  -> (idx int64 [T, k], weight fp16 [T, k])."""
+    p = torch.softmax(logits16.float(), dim=-1)
+    w, idx = torch.topk(p, k, dim=-1)
+    return idx, (w / w.sum(-1, keepdim=True)).half()
+
+
+# The fp32 rule's window.  The device expf is within 2 fp32 ulps of exp (CUDA C Programming Guide, its maximum ulp error),
+# numpy's float32 exp within 2.5 (measured over [-40, 0]); EXPF_REL = 8 ulps = 2^-20 covers the two with room.  Everything
+# else the kernel computes exactly as kernel_scores_f32 does, so a score moves by at most
+#   numerator EXPF_REL, denominator EXPF_REL on the exact sum plus (E - 1) u of the sequential fp32 sum on each side,
+#   the division u on each side:                      W(E) = 2 EXPF_REL + 2 E u            (u = 2^-24, relative)
+# and a weight score / sum, the fp32 sum of k scores:  2 W(E) + 2 k u.
+EXPF_REL = 2.0 ** -20
+
+
+def route_f32_window(E):
+    return 2 * EXPF_REL + 2 * E * 2.0 ** -24
+
+
+def route_weight_window(E, k):
+    return 2 * route_f32_window(E) + 2 * k * 2.0 ** -24
+
+
+def route_f32_explains(lg16, se, sw16, k):
+    """True when slot_expert se [k] / slot_weight sw16 [k] (fp16 bits, int16) of one token are a moe_route_kernel<true>
+    outcome for fp16 logits lg16 [E] whose exponentials differ from numpy's within EXPF_REL: expert se[j] may stand where the
+    scores give another only when the two fp32 scores lie within the window W(E) of each other (the scan is greedy, so
+    every pick is judged against every expert not picked before it), and a weight may take the other fp16 rounding of
+    score / sum only when that quotient lies within the weight window of an fp16 midpoint."""
+    sc = kernel_scores_f32(lg16.reshape(1, -1))[0].astype(np.float64)
+    E = sc.shape[0]
+    W, RW = route_f32_window(E), route_weight_window(E, k)
+    se = [int(e) for e in se]
+    if len(set(se)) != k or not all(0 <= e < E for e in se):
+        return False
+    for j, e in enumerate(se):
+        rest = [o for o in range(E) if o not in se[:j + 1]]
+        if any(sc[o] - sc[e] > W * (sc[o] + sc[e]) for o in rest):
+            return False
+    val = sc[se].astype(np.float32)
+    s = np.float32(0)
+    for v in val:
+        s = np.float32(s + v)
+    r = torch.from_numpy((val / s).astype(np.float32).astype(np.float64))
+    near, alt, dist = fp16_sides(r)
+    got = torch.from_numpy(np.asarray(sw16, dtype=np.int16).view(np.float16).astype(np.float64))
+    ok = (got == near) | ((got == alt) & (dist <= RW * r.abs()))
+    return bool(ok.all())
 
 
 # ------------------------------------------------------------------------------------- decode attention model --------
@@ -282,12 +357,7 @@ def logit_window(xn, gate):
 
 def route_scores32(logits16):
     """fp16 [T, E] logits -> the kernel's fp32 softmax scores (experts summed in index order) as float64, unrounded."""
-    lg = logits16.float().cpu().numpy()
-    ex = np.exp((lg - lg.max(-1, keepdims=True)).astype(np.float32)).astype(np.float32)
-    den = np.zeros(lg.shape[0], dtype=np.float32)
-    for e in range(lg.shape[1]):
-        den = (den + ex[:, e]).astype(np.float32)
-    return torch.from_numpy((ex / den[:, None]).astype(np.float32)).double()
+    return torch.from_numpy(kernel_scores_f32(logits16)).double()
 
 
 def route_check(xn, gate, sw, se, k, max_amb=MAX_AMB):
@@ -317,6 +387,39 @@ def route_check(xn, gate, sw, se, k, max_amb=MAX_AMB):
         s = route_scores32(lg16)
         _, _, sd = fp16_sides(s)
         assert bool((sd <= 2.0 ** -20 * s.abs()).any()), (t, se_c[t].tolist(), idx[:4].tolist())
+        window += 1
+    return matched, window, skipped
+
+
+def route_check_f32(xn, gate, sw, se, k, max_amb=MAX_AMB):
+    """route_check for the fp32 score rule (moe_route_kernel<true>): every token's slot_expert / slot_weight [T, k] must be
+    a kernel_route_f32 outcome, bit for bit, for some fp16 rounding of its ambiguous logits, or one that
+    route_f32_explains within the expf window -> (tokens matched bit for bit, tokens in the window, tokens with too many
+    ambiguous logits)."""
+    L, R = logit_window(xn, gate)
+    near, alt, dist = fp16_sides(L)
+    amb = (dist <= R).cpu()
+    near, alt = near.cpu(), alt.cpu()
+    se_c, sw_c = se.cpu().long(), _bits16(sw).cpu()
+    matched = window = skipped = 0
+    for t in range(L.shape[0]):
+        ai = torch.nonzero(amb[t]).reshape(-1).tolist()
+        if len(ai) > max_amb:
+            skipped += 1
+            continue
+        combos = torch.tensor(list(itertools.product([0, 1], repeat=len(ai))), dtype=torch.bool).reshape(2 ** len(ai), len(ai))
+        C = near[t].repeat(combos.shape[0], 1)
+        if ai:
+            C[:, ai] = torch.where(combos, alt[t, ai][None].expand_as(combos), near[t, ai][None].expand_as(combos))
+        lg16 = C.half()
+        idx, w = kernel_route_f32(lg16, k)
+        hit = (idx == se_c[t][None]).all(1) & (w.view(torch.int16) == sw_c[t][None]).all(1)
+        if bool(hit.any()):
+            matched += 1
+            continue
+        assert any(route_f32_explains(lg16[c], se_c[t].numpy(), sw_c[t].numpy(), k) for c in range(lg16.shape[0])), (
+            t, "fp32 rule", se_c[t].tolist(), sw_c[t].view(torch.float16).tolist(), idx[:4].tolist(),
+            w[:4].float().tolist())
         window += 1
     return matched, window, skipped
 

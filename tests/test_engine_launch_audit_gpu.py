@@ -19,15 +19,21 @@ teacher-forced, so an error is the launch's own.  `ws` is scratch.
   gemv SILU / QKV  an F16 launch on the cloned inputs gives y (held to the bound); act, q and the K / V cache slots must
                    follow from y bit for bit.  K / V land at cache row row0 + t // tokens_per_seq, position pos[t], of the
                    current layer; every other element of both caches keeps its bytes
+  bias (internlm)  QKV with B200_BIAS_ACC: the F16 relaunch carries the same bias, y is held to the bound of
+                   x . w_hat + b widened by the one fp32 add (BIAS_ADD_REL, Audit._y_bound), q / K / V follow from y bit
+                   for bit.  wo with B200_BIAS_OUT: the launch without the bias gives y0 (held to the bound), and
+                   o = fp16(y0 + b) bit for bit.  A bias on any other launch, or the other mode, fails
   attn_decode      the float64 bound of test_attn_decode_gpu.py on the cache rows of the chunk's sequences; counters back
                    at zero
   moe_route        h_out bit for bit, xn_out one candidate, slot_expert / slot_weight a kernel_route outcome of the logit
-                   window of its own xn_out (section B)
+                   window of its own xn_out (section B); with scores_f32 (mixtral_sparse, which must pass it, and only
+                   it) a kernel_route_f32 outcome, or one inside the expf window (oracle.numerics.route_check_f32)
   moe_expert_ffn   section B ranges for act and the bound for y_slot, on every slot routed to a local expert
   moe_combine      bit for bit
   _head            the F32 bound, and its rows are the last token of every sequence (or every row of a decode step)
 Every launch: no engine buffer changes outside the output elements its checker verified (the declared rows, and within
-them the declared columns), and a launch kind without a checker fails.
+them the declared columns), and a launch kind without a checker fails, as does an argument its checker does not take
+(no checker swallows keyword arguments: a new epilogue argument fails the audit until a checker checks it).
 
 The tensor-core prompt path (_prefill_chunk_tc: one sequence, <= 256 positions per chunk, every intermediate materialised,
 so no checker re-launches anything):
@@ -41,7 +47,8 @@ so no checker re-launches anything):
                    computed exactly from each candidate rstd.
   prefill_gemm_w4  (W4, W3, fp16) |out - ref| <= ulp16(ref) + C_ACC |x| . |w_hat|^T elementwise (test_prefill_gpu.py),
                    ref = float64 x . w_hat^T with w_hat = fp16(fp16(q - z) s) rebuilt from the engine's PackedLinear bytes
-                   (the weight itself for fp16), in blocks of output rows; out rows >= T keep their bytes
+                   (the weight itself for fp16), in blocks of output rows; out rows >= T keep their bytes.  internlm's
+                   biases as for the GEMV: ACC around ref + b, OUT through a relaunch without the bias
   prefill_rope_kv  q_out = qkv_from_y(qkv rows) bit for bit; K / V at cache row row0 (the chunk's sequence), position
                    pos[t], of the current layer; every other cache byte (other sequences' rows too) keeps its value
   prefill_silu_mul bit for bit outside the SILU_REL band (Mixtral: T k slot rows of the experts' width fe)
@@ -58,6 +65,7 @@ differs from the route of the float64 logits of its own input, with the float64 
 """
 import contextlib
 import ctypes as C
+import inspect
 import math
 import os
 
@@ -73,8 +81,9 @@ from llama2_accessory_b200.engine import DecodeEngine, EngineConfig  # noqa: E40
 from oracle import cases, omniquant, weights  # noqa: E402
 from oracle.llama_port import PortModel  # noqa: E402
 from oracle.numerics import (C_ACC, SILU_REL, TUNE_DEFAULTS, AttnRef, attn_host_split, fp16_sides,  # noqa: E402
-                             gemv_check, gemv_tol, kernel_route, logit_window, qkv_from_y, route_check,
-                             rstd_candidates, silu_mul_range, x_candidates)
+                             gemv_check, gemv_tol, kernel_route, kernel_route_f32, logit_window, qkv_from_y,
+                             route_check, route_check_f32, route_scores32, rstd_candidates, silu_mul_range,
+                             x_candidates)
 from test_prefill_moe_gpu import BAND_ABS, BAND_FACTOR  # noqa: E402
 
 DEV = "cuda"
@@ -84,6 +93,8 @@ BUFS = ("h0", "h1", "q", "attn", "o", "f", "act", "xn", "slot_w", "slot_e", "act
 PBUFS = ("p_h0", "p_h1", "p_x", "p_qkv", "p_q", "p_attn", "p_o", "p_gu", "p_act", "p_f", "p_pos", "p_tok", "p_slot_w",
          "p_slot_e", "p_y_slot")
 SHARED = ("logits_loc", "kcache", "vtcache", "counters")  # the only GEMV-path buffers a tensor-core chunk may write
+# the one extra fp32 rounding of a B200_BIAS_ACC launch, relative to |float64 x . w_hat + b| (Audit._y_bound)
+BIAS_ADD_REL = 2.0 ** -23
 MIXTRAL_WIDTH = dict(dim=4096, hidden_dim=14336, n_layers=1, n_heads=32, n_kv_heads=8, norm_eps=1e-5, rope_theta=1e6,
                      vocab_size=2048, max_seq_len=64, max_batch_size=2, moe=dict(num_experts=8, num_experts_per_tok=2))
 
@@ -170,9 +181,11 @@ class Audit:
         self.flips = []            # routing decisions that differ from the float64 route of their own input
         self.ties = 0              # tokens routed with two exactly equal float64 gate logits
         self.routed = 0            # tokens routed
+        self.route_window = 0      # tokens routed inside the expf window rather than bit for bit
         self.queue, self.ctx = [], None
         self.layer, self.resid, self.delta = -1, None, None
         self.n_engine = 0          # launch_count increments inside audited engine launches
+        self.n_checker = 0         # launch_count increments of the checkers' own relaunches
         self.start_pos = 0
         self.even = int(os.environ.get("B200_ATTN_EVEN", TUNE_DEFAULTS["B200_ATTN_EVEN"]))
         self.tc = False            # inside a _prefill_chunk_tc call
@@ -231,9 +244,10 @@ class Audit:
             self.w_hat_cache[id(pl)] = (pl, _w_hat(pl))
         return self.w_hat_cache[id(pl)][1]
 
-    def gemm_check(self, out, X, pl, label):
+    def gemm_check(self, out, X, pl, label, bias=None):
         """out [n, N] fp16 against float64 X [n, K] . w_hat^T with the prompt GEMM's bound, in blocks of output rows (a
-        70B-width w13's w_hat is 3.8 GB in float64) -> worst err / tol."""
+        70B-width w13's w_hat is 3.8 GB in float64) -> worst err / tol.  bias (B200_BIAS_ACC, out = fp16(fl32(acc + b))):
+        ref + b, and the one extra fp32 rounding of the add, BIAS_ADD_REL |ref + b| (as Audit._y_bound derives it)."""
         W = self.w_hat(pl)
         assert torch.isfinite(out).all(), label
         Xd = X.double()
@@ -243,8 +257,12 @@ class Audit:
         for n0 in range(0, pl.N, blk):
             w = W[n0:n0 + blk].double()
             ref, mag = Xd @ w.T, Xa @ w.abs().T
+            tol = C_ACC * mag
+            if bias is not None:
+                ref = ref + bias[n0:n0 + blk].double()[None]
+                tol = tol + BIAS_ADD_REL * ref.abs()
             err = (out[:, n0:n0 + blk].double() - ref).abs()
-            worst = max(worst, float((err / (_ulp16(ref) + C_ACC * mag)).max()))
+            worst = max(worst, float((err / (_ulp16(ref) + tol)).max()))
         assert worst <= 1.0, (label, worst)
         return worst
 
@@ -290,6 +308,10 @@ class Audit:
             torch.cuda.synchronize()
             check = getattr(self, "check_" + kind, None)
             assert check is not None, f"launch {kind} has no checker: the audit does not know what it may write"
+            try:
+                inspect.signature(check).bind(before, *a, **kw)
+            except TypeError as err:
+                raise AssertionError(f"launch {kind}: an argument its checker does not check ({err})") from None
             declared = check(before, *a, **kw)
             self.no_stray_writes(kind, before, declared)
             for n in declared:
@@ -459,32 +481,66 @@ class Audit:
         self.resid = other
         return b[other][:T].clone(), {other: T}
 
-    def _y_bound(self, y, h, gamma, eps, pl):
-        """y [T, N] (fp16 or fp32) against float64 for the best rstd candidate of every row -> worst err / tol."""
+    def _y_bound(self, y, h, gamma, eps, pl, bias=None):
+        """y [T, N] (fp16 or fp32) against float64 for the best rstd candidate of every row -> worst err / tol.
+
+        bias (B200_BIAS_ACC): y = fp16(fl32(acc + b)) against Y = x . w_hat + b.  With |acc - x . w_hat| <= C_ACC M the
+        extra fp32 add rounds once, fl32(acc + b) = (acc + b)(1 + d), |d| <= 2^-24, so |fl32(acc + b) - Y| <=
+        C_ACC M (1 + 2^-24) + 2^-24 |Y|, and the fp16 rounding adds half an ulp of a value within (1 + 2^-23) |Y| +
+        2 C_ACC M.  The GEMV bound (gemv_tol: 2^-11 |Y| + C_ACC M (1 + 2^-10) + 2^-25) covers all of it but the
+        2^-24 |Y| (1 + 2^-11) + 2^-35 |Y| of the add, which BIAS_ADD_REL |Y| = 2^-23 |Y| covers."""
         W, A = self.dense(pl)
+        b = None if bias is None else bias.double()
         worst = 0.0
         for t in range(y.shape[0]):
             X = x_candidates(h[t], gamma, eps).double()
             Y, M = X @ W.T, X.abs() @ A.T
-            r = ((y[t].double()[None] - Y).abs() / gemv_tol(Y, M)).amax(1)
+            tol = gemv_tol(Y, M)
+            if b is not None:
+                Y = Y + b[None]
+                tol = gemv_tol(Y, M) + BIAS_ADD_REL * Y.abs()
+            r = ((y[t].double()[None] - Y).abs() / tol).amax(1)
             worst = max(worst, float(r.min()))
         assert worst <= 1.0, (self.layer, pl.N, pl.K, worst)
         return worst
 
-    def _f16_relaunch(self, pl, T, resid, delta, gamma, eps):
-        y = torch.empty(T, pl.N, dtype=torch.float16, device=DEV)
+    def _relaunch(self, name, *a, **kw):
+        """A checker's own launch of the real entry point `name`, synchronised and counted apart from the engine's."""
         n0 = ops.launch_count
-        self.real["gemv"](pl, T, out=y, epilogue=ops.B200_EPI_F16, resid=resid, delta=delta, gamma=gamma, eps=eps)
+        self.real[name](*a, **kw)
         torch.cuda.synchronize()
-        assert ops.launch_count == n0 + 1
+        self.n_checker += ops.launch_count - n0
+
+    def _f16_relaunch(self, pl, T, resid, delta, gamma, eps, bias=None, bias_mode=ops.B200_BIAS_NONE):
+        y = torch.empty(T, pl.N, dtype=torch.float16, device=DEV)
+        n0 = self.n_checker
+        self._relaunch("gemv", pl, T, out=y, epilogue=ops.B200_EPI_F16, resid=resid, delta=delta, gamma=gamma, eps=eps,
+                       bias=bias, bias_mode=bias_mode)
+        assert self.n_checker == n0 + 1
         return y
 
+    def _bias_role(self, lin, bias, bias_mode):
+        """The bias a launch of `lin` must carry: internlm's Wqkv bias before RoPE (B200_BIAS_ACC, one rounding of acc + b)
+        and its out_proj bias on the fp16 output (B200_BIAS_OUT); none on any other linear, or on a model without them."""
+        lw = self.eng.layers[self.layer]
+        want = {id(lw.wqkv): (lw.bqkv, ops.B200_BIAS_ACC), id(lw.wo): (lw.bo, ops.B200_BIAS_OUT)}.get(id(lin), (None, None))
+        if want[0] is None:
+            assert bias is None and bias_mode in (None, ops.B200_BIAS_NONE), (self.layer, "a bias this linear does not have")
+            return None
+        assert bias is want[0] and bias_mode == want[1], (self.layer, "bias / bias_mode", bias_mode, "expected", want[1])
+        return bias
+
     def check_gemv(self, before, lin, T, *, out, epilogue=ops.B200_EPI_F16, xin=None, resid=None, delta=None, h_out=None,
-                   gamma=None, eps=1e-5, qkv=None, moe=None, **kw):
+                   gamma=None, eps=1e-5, qkv=None, moe=None, use_pdl=False, ring_bytes=0, prefetch=None, ar=None,
+                   prefetch_const=None, bias=None, bias_mode=ops.B200_BIAS_NONE):
+        """use_pdl, ring_bytes, prefetch and prefetch_const change nothing a launch computes (test_decode_path_gpu.py holds
+        them to bit identity); every other argument is checked."""
         e, x = self.eng, self.ctx
-        assert moe is None and kw.get("ar") is None, "moe-slot / fused all-reduce gemv: no checker"
+        assert moe is None and ar is None, "moe-slot / fused all-reduce gemv: no checker"
+        if epilogue not in (ops.B200_EPI_QKV, ops.B200_EPI_F16):
+            assert bias is None and bias_mode == ops.B200_BIAS_NONE, "a bias on a gemv epilogue without a bias checker"
         if epilogue == ops.B200_EPI_QKV:
-            return self._check_qkv(before, lin, T, out, resid, delta, h_out, gamma, eps, qkv)
+            return self._check_qkv(before, lin, T, out, resid, delta, h_out, gamma, eps, qkv, bias, bias_mode)
         if epilogue == ops.B200_EPI_SILU:
             assert self.c.kind == "llama" and lin is e.layers[self.layer].w13 and self.name(out) == "act"
             rb, db = resid.clone(), delta.clone()
@@ -518,31 +574,47 @@ class Audit:
             assert lin is lw.w2 and (src, dst) == ("act", "f")
             kind = "gemv F16 (w2)"
             self.delta = "f"
+        b = self._bias_role(lin, bias, bias_mode)
         W, A = self.dense(lin)
         xd = xin[:T, :lin.K].double()
-        r, _, _ = gemv_check(out[:T], xd @ W.T, xd.abs() @ A.T, (kind, self.layer))
+        y = out[:T]
+        if b is not None:
+            # B200_BIAS_OUT: the launch without the bias gives y0 (held to the bound); out = fp16(y0 + b) bit for bit
+            y = torch.empty(T, lin.N, dtype=torch.float16, device=DEV)
+            self._relaunch("gemv", lin, T, xin=xin, out=y, epilogue=ops.B200_EPI_F16, use_pdl=use_pdl,
+                           ring_bytes=ring_bytes, prefetch=prefetch, prefetch_const=prefetch_const)
+            assert _same(out[:T], (y.float() + b.float()[None]).half()), (self.layer, kind, "out != fp16(y0 + b)")
+            kind += " BIAS_OUT"
+        r, _, _ = gemv_check(y, xd @ W.T, xd.abs() @ A.T, (kind, self.layer))
         self.note(kind, r)
         return {dst: T}
 
-    def _check_qkv(self, before, lin, T, out, resid, delta, h_out, gamma, eps, qkv):
+    def _check_qkv(self, before, lin, T, out, resid, delta, h_out, gamma, eps, qkv, bias, bias_mode):
+        """The F16 relaunch carries the launch's own bias (B200_BIAS_ACC: y = fp16(acc + b), the value RoPE starts from),
+        so q and K / V follow from y bit for bit with or without one; y is held to the bound of x . w_hat (+ b)."""
         e, x = self.eng, self.ctx
         self.layer += 1
         i, row0, tps = self.layer, x["row0"], x["tps"]
         lw = e.layers[i]
         assert lin is lw.wqkv and gamma is lw.attn_norm and self.name(out) == "q"
+        b = self._bias_role(lin, bias, bias_mode)
         assert qkv["tokens_per_seq"] == tps and qkv["pos"].data_ptr() == e.pos.data_ptr() and qkv["rope"] is e.rope
         assert qkv["kcache"].data_ptr() == e.kcache[i, row0].data_ptr(), ("K cache slice", i, row0)
         assert qkv["vtcache"].data_ptr() == e.vtcache[i, row0].data_ptr(), ("V cache slice", i, row0)
+        assert set(qkv) <= {"n_q_rows", "n_kv_rows", "rope", "pos", "tokens_per_seq", "kcache", "vtcache", "cache_seq",
+                            "prefetch_kv"} and qkv["cache_seq"] == e.cache_seq, sorted(qkv)
         rb, db = resid.clone(), None if delta is None else delta.clone()
         h, decl = self._prologue(resid, delta, h_out, T)
-        y = self._f16_relaunch(lin, T, rb, db, gamma, eps)
-        r = self._y_bound(y, h, gamma, eps, lin)
+        y = self._f16_relaunch(lin, T, rb, db, gamma, eps, bias=b, bias_mode=bias_mode if b is not None else
+                               ops.B200_BIAS_NONE)
+        r = self._y_bound(y, h, gamma, eps, lin, bias=b)
         nq, nkv = qkv["n_q_rows"], qkv["n_kv_rows"]
+        assert (nq, nkv) == (e.Hq * 128, e.Hkv * 128)
         pos = x["pos"]
         q, k, v = qkv_from_y(y, e.rope, pos, nq, nkv)
         assert _same(out[:T], q), (i, "q != RoPE(y)")
         self._kv_written(before, [row0 + t // tps for t in range(T)], pos, k, v)
-        self.note("gemv QKV", r)
+        self.note("gemv QKV BIAS_ACC" if b is not None else "gemv QKV", r)
         return dict(decl, q=T, kcache="checked", vtcache="checked")
 
     def _kv_written(self, before, rows, pos, k, v):
@@ -560,8 +632,9 @@ class Audit:
         assert _same(e.vtcache, vexp), (i, rows[0], "V cache: a slot other than (row, pos[t]) or a wrong value")
 
     def check_attn_decode(self, before, q, kcache, vtcache, pos, out, *, T, Hq, Hkv, cache_seq, tokens_per_seq, max_kv_len,
-                          ws=None, counters=None, n_split=0, **kw):
+                          ws=None, counters=None, n_split=0, scale=None, use_pdl=False, prefetch=None):
         e, x = self.eng, self.ctx
+        assert scale is None, "attention scale other than 1 / sqrt(128): the float64 bound assumes that one"
         i, row0 = self.layer, x["row0"]
         t0, tps, kind = 0, x["tps"], "attn_decode"
         if self.tc:
@@ -593,11 +666,15 @@ class Audit:
         return {"attn": T}
 
     def check_moe_route(self, before, *, T, D, E, topk, resid, delta, h_out, gamma, eps, gate_w, xn_out, slot_weight,
-                        slot_expert, **kw):
+                        slot_expert, use_pdl=False, scores_f32=False):
+        """scores_f32 must be the model's rule (mixtral_sparse: fp32, route_check_f32; Mixtral: fp16, route_check); the
+        float64 flip report routes the float64 logits by the same rule."""
         e, x = self.eng, self.ctx
         i, k = self.layer, topk
         lw = e.layers[i]
         assert gate_w is lw.gate and gamma is lw.ffn_norm and T == x["T"]
+        assert bool(scores_f32) == e.cfg.sparse_moe and scores_f32 in (0, 1, False, True), ("score rule", scores_f32)
+        assert (D, E, topk) == (e.cfg.dim, e.cfg.num_experts, e.cfg.experts_per_tok)
         xn_n, sw_n, se_n = self.p("x") if self.tc else "xn", self.p("slot_w"), self.p("slot_e")
         assert (self.name(xn_out), self.name(slot_weight), self.name(slot_expert)) == (xn_n, sw_n, se_n)
         if self.tc:
@@ -608,28 +685,32 @@ class Audit:
             X = x_candidates(h[t], gamma, eps)
             assert bool((_raw(X) == _raw(xn[t])[None]).all(1).any()), (i, t, "xn_out is no candidate of the rstd window")
         se, sw = slot_expert[:T * k].view(T, k), slot_weight[:T * k].view(T, k)
-        matched, window, skipped = route_check(xn, gate_w, sw, se, k)
+        check, route = (route_check_f32, kernel_route_f32) if scores_f32 else (route_check, kernel_route)
+        matched, window, skipped = check(xn, gate_w, sw, se, k)
         assert skipped == 0 and matched + window == T
+        self.route_window += window
         # the float64 route of the same input: logits rounded to nearest fp16, then the kernel's routing rule
         L, R = logit_window(xn, gate_w)
-        near = fp16_sides(L)[0]
-        idx64, _ = kernel_route(near.half().cpu(), k)
+        near = fp16_sides(L)[0].half().cpu()
+        idx64, _ = route(near, k)
         p64 = torch.softmax(L, -1).cpu()
+        s32 = route_scores32(near)
         se_c = se.cpu().long()
         for t in torch.nonzero((idx64 != se_c).any(1)).reshape(-1).tolist():
             j = int(torch.nonzero(idx64[t] != se_c[t])[0])
             a, b = int(se_c[t, j]), int(idx64[t, j])
             self.flips.append(dict(start_pos=self.start_pos, layer=i, seq=x["seq"][t], pos=x["pos"][t],
-                                   kernel=se_c[t].tolist(), float64=idx64[t].tolist(),
-                                   gap=float(p64[t, a] - p64[t, b]), logit_gap=float(L[t, a] - L[t, b]),
-                                   window=float(R[t, a] + R[t, b])))
+                                   kernel=se_c[t].tolist(), float64=idx64[t].tolist(), rule="fp32" if scores_f32 else "fp16",
+                                   gap=float(p64[t, a] - p64[t, b]), gap32=float(s32[t, a] - s32[t, b]),
+                                   logit_gap=float(L[t, a] - L[t, b]), window=float(R[t, a] + R[t, b])))
         Lc = L.cpu()
         self.ties += sum(int(Lc[t].unique().numel() < Lc.shape[1]) for t in range(T))
         self.routed += T
-        self.note("moe_route (tensor-core chunk)" if self.tc else "moe_route", 0.0)
+        kind = "moe_route" + (" fp32 rule" if scores_f32 else "")
+        self.note(kind + (" (tensor-core chunk)" if self.tc else ""), 0.0)
         return dict(decl, **{xn_n: T, sw_n: T * k, se_n: T * k})
 
-    def check_moe_expert_ffn(self, before, w13, w2, *, T, D, F, topk, e_first, xn, slot_expert, act, y_slot, **kw):
+    def check_moe_expert_ffn(self, before, w13, w2, *, T, D, F, topk, e_first, xn, slot_expert, act, y_slot, use_pdl=False):
         e = self.eng
         lw = e.layers[self.layer]
         assert w13 == lw.e_w13 and w2 == lw.e_w2 and e_first == e.e_first and F == e.F
@@ -705,7 +786,10 @@ class Audit:
         self.note("prefill_rmsnorm", 0.0)
         return dict(decl, p_x=T)
 
-    def check_prefill_gemm_w4(self, before, lin, x_in, out, T):
+    def check_prefill_gemm_w4(self, before, lin, x_in, out, T, bias=None, bias_mode=None):
+        """b200_prefill_gemm_w4, or b200_prefill_gemm_w4_bias with internlm's biases: B200_BIAS_ACC (Wqkv) held to the
+        GEMM bound around ref + b; B200_BIAS_OUT (wo) relaunched without the bias to y0, y0 held to the bound and
+        out = fp16(y0 + b) bit for bit."""
         e, x = self.eng, self.ctx
         assert self.tc and T == x["T"]
         lw = e.layers[self.layer]
@@ -726,14 +810,23 @@ class Audit:
             self.delta = "p_f"
         assert (src, dst) == io, (kind, src, dst)
         self.wrote(src, producer)
+        b = self._bias_role(lin, bias, bias_mode)
         X = x_in.view(-1)[:T * lin.K].view(T, lin.K)
-        r = self.gemm_check(out.view(-1)[:T * lin.N].view(T, lin.N), X, lin, (self.layer, kind))
+        got = out.view(-1)[:T * lin.N].view(T, lin.N)
+        if b is not None and bias_mode == ops.B200_BIAS_OUT:
+            y0 = torch.empty(T, lin.N, dtype=torch.float16, device=DEV)
+            self._relaunch("prefill_gemm_w4", lin, x_in, y0, T)
+            assert _same(got, (y0.float() + b.float()[None]).half()), (self.layer, kind, "out != fp16(y0 + b)")
+            r = self.gemm_check(y0, X, lin, (self.layer, kind))
+        else:
+            r = self.gemm_check(got, X, lin, (self.layer, kind), bias=b)
         if self.hidden is not None and kind in ("wo", "w2"):
             # the residual after the block's attention (wo) or after the block (w2), as the next prologue forms it
             h = (self.bufs()[self.resid][:T] + out[:T]).float().cpu()
             for t in range(T):
                 self.hidden[(self.start_pos, self.layer, "attn" if kind == "wo" else "block", x["seq"][t], x["off"][t])] = h[t]
-        self.note(f"prefill_gemm_w4 ({'fp16' if lin.bits == 16 else f'W{lin.bits}'} {kind})", r)
+        tag = "" if b is None else " BIAS_OUT" if bias_mode == ops.B200_BIAS_OUT else " BIAS_ACC"
+        self.note(f"prefill_gemm_w4 ({'fp16' if lin.bits == 16 else f'W{lin.bits}'} {kind}{tag})", r)
         return {dst: ("flat", T * lin.N)}
 
     def check_prefill_rope_kv(self, before, qkv, q_out, kcache, vtcache, rope, pos, T, n_q_rows, n_kv_rows, tokens_per_seq,
@@ -799,27 +892,25 @@ class Audit:
     def run(self, toks, calls):
         """calls: [(start_pos, length)] in order over toks [bsz, *] (CPU)."""
         with self.installed():
-            lc0, n0 = ops.launch_count, self.n_engine
+            lc0, n0, c0 = ops.launch_count, self.n_engine, self.n_checker
             for sp, n in calls:
                 chunk = toks[:, sp:sp + n].contiguous()
                 self.expect(chunk, sp)
                 assert torch.isfinite(self.eng.forward_inference(chunk.to(DEV), sp)).all()
                 assert not self.queue, "forward_inference made fewer _step calls than its schedule"
             checker_launches = ops.launch_count - lc0 - (self.n_engine - n0)
-        assert checker_launches == self.stats.get("gemv QKV", [0])[0] + self.stats.get("gemv SILU (w13)", [0])[0], \
-            "a launch outside the audited entry points"
+        assert checker_launches == self.n_checker - c0, "a launch outside the audited entry points"
 
     def run_full(self, toks, forward):
         """forward(tokens) -> [bsz, seqlen, vocab] fp16 through DecodeEngine.forward_full, every launch audited; every
         chunk's rows of the output must equal fp16 of the logits its audited _head launch wrote."""
         with self.installed():
-            lc0, n0 = ops.launch_count, self.n_engine
+            lc0, n0, c0 = ops.launch_count, self.n_engine, self.n_checker
             self.expect_full(toks)
             out = forward(toks.to(DEV))
             assert not self.queue, "forward_full made fewer _step calls than its schedule"
             checker_launches = ops.launch_count - lc0 - (self.n_engine - n0)
-        assert checker_launches == self.stats.get("gemv QKV", [0])[0] + self.stats.get("gemv SILU (w13)", [0])[0], \
-            "a launch outside the audited entry points"
+        assert checker_launches == self.n_checker - c0, "a launch outside the audited entry points"
         assert out.shape == (*toks.shape, self.c.vocab_size) and out.dtype == torch.float16
         for e in self.done:
             b0, nb, off, ci = e["row0"], e["nb"], e["off0"], e["ci"]
@@ -832,13 +923,14 @@ class Audit:
         lines = [f"\n[audit {label}]"]
         for k, (n, w) in sorted(self.stats.items()):
             lines.append(f"  {k:40s} {n:6d} launches, worst err/tol {w:.3f}")
-        if "moe_route" in self.stats:
-            lines.append(f"  tokens routed with two exactly equal gate logits: {self.ties}")
+        if self.routed:
+            lines.append(f"  tokens routed with two exactly equal gate logits: {self.ties}; routed inside the expf window "
+                         f"(not bit for bit): {self.route_window} of {self.routed}")
         lines.append(f"  routing decisions differing from the float64 route of their own input: {len(self.flips)}")
         for f in self.flips:
-            lines.append(f"    start {f['start_pos']} layer {f['layer']} seq {f['seq']} pos {f['pos']}: kernel {f['kernel']} "
-                         f"float64 {f['float64']}, float64 score gap {f['gap']:.3e}, logit gap {f['logit_gap']:.3e} "
-                         f"(window {f['window']:.3e})")
+            lines.append(f"    start {f['start_pos']} layer {f['layer']} seq {f['seq']} pos {f['pos']} ({f['rule']} rule): "
+                         f"kernel {f['kernel']} float64 {f['float64']}, float64 score gap {f['gap']:.3e}, fp32 score gap "
+                         f"{f['gap32']:.3e}, logit gap {f['logit_gap']:.3e} (window {f['window']:.3e})")
         print("\n".join(lines))
         assert all(w <= 1.0 for _, w in self.stats.values())
 

@@ -1,8 +1,10 @@
 """CPU: `mixtral_sparse` models (accessory/model/LLM/mixtral_sparse.py) -- every expert sliced over the tensor-parallel
 ranks, and the fp32 router rule.
 
-  * the fp32 router, restated, against the routing of the unmodified module (run through oracle/shims/{megablocks,stk}),
-    including logits where the fp16 rule of base Mixtral and the fp32 rule pick different experts;
+  * the fp32 router, restated in torch (oracle.numerics.route_f32), against the routing of the unmodified module (run
+    through oracle/shims/{megablocks,stk}), including logits where the fp16 rule of base Mixtral and the fp32 rule pick
+    different experts; the line-by-line model of the kernel's fp32 rule (kernel_route_f32) against that statement wherever
+    no near-tie exists, and its window (route_f32_explains);
   * the port (oracle/sparse.py) against the unmodified module, and the committed goldens against both;
   * checkpoint merge / split between checkpoint TP 1, 2, 4, 8 and engine TP 1, 2, 4, 8 against the module's own
     _sparse_expert_merge / _sparse_expert_split; the per-expert view the engine loads from; packed-shard config;
@@ -22,7 +24,8 @@ import llama2_accessory_b200 as pkg
 from llama2_accessory_b200 import _cabi, checkpoint, ops
 from llama2_accessory_b200.engine import DecodeEngine, EngineConfig, check_kernel_limits
 from oracle import cases, ref_import, sparse
-from oracle.numerics import kernel_route
+from oracle.numerics import (fp16_sides, kernel_route, kernel_route_f32, kernel_scores_f32, route_f32, route_f32_explains,
+                             route_f32_window, route_weight_window)
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 # the unmodified mixtral_sparse.py is read from the reference tree; the staged copy of the hot-path modules does not include it
@@ -31,14 +34,6 @@ needs_ref = pytest.mark.skipif(
     reason="needs the reference tree's accessory/model/LLM/mixtral_sparse.py")
 MIX = dict(dim=4096, n_heads=32, n_kv_heads=8, vocab_size=32000, hidden_dim=14336, rope_theta=1e6,
            moe=dict(num_experts=8, num_experts_per_tok=2))
-
-
-def route_f32(logits16, k):
-    """mixtral_sparse.py:417-428 on fp16 logits [T, E]: fp32 softmax, top-k on the fp32 scores (ties: lower index),
-    fp32 renormalisation, one cast to fp16.  -> (idx int64 [T, k], weight fp16 [T, k])."""
-    p = torch.softmax(logits16.float(), dim=-1)
-    w, idx = torch.topk(p, k, dim=-1)
-    return idx, (w / w.sum(-1, keepdim=True)).half()
 
 
 def _ref_moe_routes(x16, gate16, k, hidden=128):
@@ -109,6 +104,94 @@ def test_crafted_logits_where_the_fp16_and_fp32_rules_disagree():
     assert differ, "no crafted row separates the two rules"
     for t in differ:
         assert list(idx16[t]) == [0, 1] and idx32[t].tolist() == [0, 2]
+
+
+def _near_ties(lg16, k):
+    """Tokens where two statements of the fp32 rule may part legitimately: two of the top k + 1 fp32 scores within the
+    window route_f32_window of each other, or a weight's score / sum within route_weight_window of an fp16 midpoint."""
+    sc = kernel_scores_f32(lg16).astype(np.float64)
+    E = sc.shape[1]
+    W, RW = route_f32_window(E), route_weight_window(E, k)
+    top = -np.sort(-sc, -1)[:, :k + 1]
+    close = ((top[:, :-1] - top[:, 1:]) <= W * (top[:, :-1] + top[:, 1:])).any(-1)
+    r = top[:, :k] / top[:, :k].sum(-1, keepdims=True)
+    _, _, dist = fp16_sides(torch.from_numpy(r))
+    return close | (dist.numpy() <= 2 * RW * r).any(-1)
+
+
+def _crafted_logits(E):
+    """Rows with exact ties, ties one fp16 step apart at 2 and at the subnormal end, and the fp16-rule / fp32-rule
+    disagreements of test_crafted_logits_where_the_fp16_and_fp32_rules_disagree (first eight experts)."""
+    rows = []
+    base = [-1.0 - 0.25 * e for e in range(E)]
+    for a, b in ((2.0, 2.0), (2.0, 2.0 + 2.0 ** -9), (2.0 ** -24, 0.0), (0.5, 0.5), (3.0, 3.0 - 2.0 ** -10)):
+        for i, j in ((0, 1), (1, 0), (E - 2, E - 1), (2, E - 1)):
+            r = list(base)
+            r[i], r[j] = a, b
+            rows.append(r)
+    rows.append([0.0] * E)
+    for d in (1, 2, 3, 4):
+        rows.append(([2.0, 0.0, d * 2.0 ** -14, -2.0, -2.0, -3.0, -3.0, -4.0] + base)[:E])
+    return torch.tensor(rows, dtype=torch.float16)
+
+
+@pytest.mark.parametrize("E,k", [(8, 2), (4, 2), (16, 4)])
+def test_kernel_route_f32_matches_the_torch_statement_away_from_near_ties(E, k):
+    """kernel_route_f32 (moe_route_kernel<true> line by line) against route_f32 (mixtral_sparse.py:417-428 in torch) on
+    random logits and on crafted near-tie rows: bit for bit wherever no near-tie exists.  Exact ties go to the lower index
+    in both; the decided crafted rows separate the fp32 rule from the fp16 rule (kernel_route)."""
+    g = torch.Generator().manual_seed(E * 10 + k)
+    rand = (torch.randn(4096, E, generator=g) * 2).half()
+    crafted = _crafted_logits(E)
+    for lg, what in ((rand, "random"), (crafted, "crafted")):
+        idx, w = kernel_route_f32(lg, k)
+        idx_t, w_t = route_f32(lg, k)
+        near = _near_ties(lg, k)
+        far = ~near
+        if what == "random":
+            assert far.sum() >= 0.8 * lg.shape[0], int(far.sum())
+        elif k == 2:
+            assert far[-4:].all() and far.sum() >= 8, far  # the fp16 / fp32 disagreement rows are decided
+        assert torch.equal(idx[far], idx_t[far]), what
+        assert torch.equal(w[far].view(torch.int16), w_t[far].view(torch.int16)), what
+        # the model's own outcome is one its window explains
+        for t in range(lg.shape[0]):
+            assert route_f32_explains(lg[t], idx[t].numpy(), w[t].view(torch.int16).numpy(), k), (what, t)
+    # exact ties: the lower index first, under the fp32 rule too
+    idx, w = kernel_route_f32(crafted, k)
+    for t, row in enumerate(crafted.tolist()):
+        top = sorted(range(E), key=lambda e: (-row[e], e))[:k]
+        if row[top[0]] == row[top[1]]:
+            assert idx[t].tolist()[:2] == top[:2], (t, row, idx[t])
+    assert idx[-4:, :2].tolist() == [[0, 2]] * 4 or E < 8
+    if E >= 8:
+        assert kernel_route(crafted[-4:], k)[0][:, :2].tolist() == [[0, 1]] * 4
+
+
+def test_route_f32_window_is_not_vacuous():
+    """On random logits (E 8, top-2) the window refuses what a wrong kernel would write: a weight one fp16 step off, the
+    experts of a decided token swapped with the third, and the weights of the fp16 rule (scores rounded to fp16 before
+    the top-k and the renormalisation)."""
+    E, k = 8, 2
+    lg = (torch.randn(512, E, generator=torch.Generator().manual_seed(3)) * 2).half()
+    idx, w = kernel_route_f32(lg, k)
+    near = _near_ties(lg, k)
+    _, w16 = kernel_route(lg, k)
+    sc = kernel_scores_f32(lg)
+    refused, differ = dict(step=0, swap=0, rule16=0), 0
+    for t in np.nonzero(~near)[0][:200]:
+        wb = w[t].view(torch.int16).numpy().copy()
+        wb[0] += 1
+        refused["step"] += not route_f32_explains(lg[t], idx[t].numpy(), wb, k)
+        third = int(np.argsort(-sc[t], kind="stable")[k])
+        sw = idx[t].numpy().copy()
+        sw[k - 1] = third
+        refused["swap"] += not route_f32_explains(lg[t], sw, w[t].view(torch.int16).numpy(), k)
+        if not torch.equal(w16[t], w[t]):
+            differ += 1
+            refused["rule16"] += not route_f32_explains(lg[t], idx[t].numpy(), w16[t].view(torch.int16).numpy(), k)
+    print(f"\n[route_f32 window] refused of 200 decided tokens: {refused}; fp16-rule weights differing: {differ}")
+    assert refused["step"] == 200 and refused["swap"] == 200 and refused["rule16"] == differ > 0, (refused, differ)
 
 
 @needs_ref

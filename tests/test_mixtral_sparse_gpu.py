@@ -1,13 +1,13 @@
 """GPU: `mixtral_sparse` models on the H100 -- the fp32 router rule of moe_route_kernel at real widths, and the engine with
 every expert sliced over the tensor-parallel ranks.
 
-  * Router (D 4096, E 8, top-2, T up to 256) against a float64 restatement.  A float64 logit farther than R from an fp16
-    rounding midpoint has one possible fp16 value, the others two (R: the running-error bound of the kernel's lane chains
-    and warp tree, oracle.numerics.logit_window).  For some choice of those, the experts must be the top-2 of the fp16
-    logits (the softmax is monotone; equal logits go to the lower index) and every weight within one fp16 step of the
-    float64 weight -- except where the 2nd and 3rd logits lie within the fp32 tie band 2^-20 (their fp32 exponentials could
-    then coincide).  With scores_f32 = 0 the same launch must satisfy today's CPU model of the fp16 rule
-    (oracle.numerics.route_check, as tests/test_gemv_batched_moe_gpu.py checks it).
+  * Router (D 4096, E 8, top-2, T up to 256).  A float64 logit farther than R from an fp16 rounding midpoint has one
+    possible fp16 value, the others two (R: the running-error bound of the kernel's lane chains and warp tree,
+    oracle.numerics.logit_window).  For some choice of those, scores_f32 = 1 must give the experts and weights of
+    oracle.numerics.kernel_route_f32 (moe_route_kernel<true> line by line) bit for bit, or differ only inside the window
+    the device expf allows: experts exchanged only where their fp32 scores lie that close, a weight's other fp16 rounding
+    only where score / sum lies that close to a midpoint (route_check_f32).  With scores_f32 = 0 the same launch must
+    satisfy the CPU model of the fp16 rule (route_check, as tests/test_gemv_batched_moe_gpu.py checks it).
   * The engine against the goldens of the unmodified module and against the port (oracle/sparse.py), with the parity rule
     of tests/test_model_parity_gpu.py: GEMV-chunk prompts, tensor-core prompts, a continuation prompt, decode eager and
     from a graph.  Against the port, the port takes the engine's routes (force_routes); every route that differs from the
@@ -33,7 +33,7 @@ import llama2_accessory_b200 as pkg  # noqa: E402
 from llama2_accessory_b200 import _cabi, checkpoint, ops  # noqa: E402
 from llama2_accessory_b200.engine import DecodeEngine, EngineConfig  # noqa: E402
 from oracle import omniquant, sparse, weights  # noqa: E402
-from oracle.numerics import MAX_AMB, fp16_sides, logit_window, route_check  # noqa: E402
+from oracle.numerics import route_check, route_check_f32  # noqa: E402
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 RULE_FACTOR = 1.5  # tests/test_model_parity_gpu.py
@@ -54,39 +54,6 @@ def _ulp16(x):
 
 
 # --------------------------------------------------------------------------------------------------- router ---------
-def _route_check_f32(xn, gate, sw, se, k):
-    """slot_expert / slot_weight [T, k] of the fp32 rule against every fp16 rounding of the ambiguous logits ->
-    (tokens matched, tokens inside the fp32 tie band, tokens with more than MAX_AMB ambiguous logits)."""
-    import itertools
-    L, R = logit_window(xn, gate)
-    near, alt, dist = (x.double().cpu().numpy() for x in fp16_sides(L))
-    amb = (dist <= R.cpu().numpy())
-    se, sw = se.numpy(), sw.double().numpy()
-    matched = window = skipped = 0
-    for t in range(L.shape[0]):
-        ai = np.nonzero(amb[t])[0]
-        if len(ai) > MAX_AMB:
-            skipped += 1
-            continue
-        cand = np.repeat(near[t][None], 2 ** len(ai), 0)
-        for c, pick in enumerate(itertools.product([0, 1], repeat=len(ai))):
-            cand[c, ai] = np.where(np.array(pick, dtype=bool), alt[t, ai], near[t, ai])
-        order = np.argsort(-cand, axis=-1, kind="stable")          # equal logits: lower index first
-        want = order[:, :k]
-        s64 = np.exp(cand - cand.max(-1, keepdims=True))
-        w = np.take_along_axis(s64, want, -1)
-        w /= w.sum(-1, keepdims=True)
-        ok = (want == se[t][None]).all(-1) & (np.abs(sw[t][None] - w) <= _ulp16(w)).all(-1)
-        if ok.any():
-            matched += 1
-            continue
-        top = np.take_along_axis(cand, order, -1)
-        assert (np.abs(top[:, k - 1] - top[:, k]) < 2.0 ** -20 * np.maximum(1.0, np.abs(top[:, k]))).any(), \
-            (t, se[t], sw[t], want[:4], w[:4])
-        window += 1
-    return matched, window, skipped
-
-
 @pytest.mark.parametrize("T", [1, 16, 256])
 def test_fp32_router_at_real_widths(T):
     D, E, k = 4096, 8, 2
@@ -107,12 +74,12 @@ def test_fp32_router_at_real_widths(T):
     xn = out[1][0]
     assert torch.equal(xn, out[0][0])
     _, sw32, se32 = out[1]
-    m32, w32, s32 = _route_check_f32(xn.cuda(), gate, sw32, se32, k)
+    m32, w32, s32 = route_check_f32(xn.cuda(), gate, sw32.cuda(), se32.cuda(), k)
     assert s32 == 0 and m32 + w32 == T and m32 >= 0.9 * T, (m32, w32, s32)
     # scores_f32 = 0: today's CPU model of the fp16 rule
     matched, window, skipped = route_check(xn.cuda(), gate, out[0][1].cuda(), out[0][2].cuda(), k)
     assert matched + window == T and skipped == 0
-    print(f"\n[router T={T}] fp32 rule: {m32} matched, {w32} in the fp32 tie band; fp16 rule: {matched} bit for bit, "
+    print(f"\n[router T={T}] fp32 rule: {m32} bit for bit, {w32} in the expf window; fp16 rule: {matched} bit for bit, "
           f"{window} in the expf window")
 
 
