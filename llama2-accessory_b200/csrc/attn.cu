@@ -4,9 +4,9 @@
 // (accessory/model/LLM/llama.py:170-206).  The KV cache is stored as shared-memory images (see below), written
 // in place by the fused QKV GEMV epilogue, so a 32-position tile of K or V is one contiguous 8 KB TMA bulk copy.
 //
-// One CTA = one (split, kv-head, token).  A producer warp streams (K tile, V tile) pairs into a 6-stage
-// shared-memory ring with cp.async.bulk + mbarriers; 4 consumer warps take tiles round-robin and never meet
-// at a CTA-wide barrier in the main loop.  All n_rep query heads of the group ride in the M dimension of the
+// One CTA = one (split, kv-head, token).  A producer warp bulk-copies K and V tiles (cp.async.bulk + mbarriers) into
+// one small ring per consumer warp; the 4 consumer warps take tiles round-robin, each from its own ring, and only
+// meet (at a named barrier, without the producer) for the in-CTA merge.  All n_rep query heads of the group ride in the M dimension of the
 // HMMAs, so K/V are read once per group (never materialising repeat_kv):
 //     S[h][s]  = Q[h][:] . K[s][:]        A = Q (16 x 16 per step), B = K rows   (k-slot permutation in d)
 //     O[h][d] += P[h][s] * Vt[d][s]       A = P straight from the S accumulators (FA2 register reuse)
@@ -33,10 +33,27 @@ int tune_get(const char* name, int dflt);
 
 constexpr int kAttnWarps = 4;                 // consumer warps; one more warp produces
 constexpr int kAttnThreads = (kAttnWarps + 1) * 32;
+constexpr int kConsumerThreads = kAttnWarps * 32;
 constexpr int kTile = 32;                     // kv positions per tile
-constexpr int kStages = 6;                    // CTA-shared ring depth (6 x 16 KB: two CTAs per SM)
-constexpr int kStageBytes = 2 * kTile * 256;  // K tile + V tile = 16 KB
+constexpr int kHalfBytes = kTile * 256;       // one K tile or one V tile: 8 KB, one bulk copy, one ring slot
+// Per-warp rings.  Warp w computes tiles w, w + 4, w + 8, ... and its ring receives exactly their halves, in the order the
+// warp uses them: K(w), V(w), K(w + 4), V(w + 4), ...  Each slot has its own full / empty mbarrier and one consumer, so a
+// slot is free again as soon as its warp has read it: a K slot after the scores, a V slot after P.V.
+// Tiles are dealt from warp 0, so warp 0 never has fewer than any other warp and gets the deepest ring:
+//   5 + 3 + 3 + 3 = 14 slots x 8 KB = 112 KB per CTA; two CTAs per SM: 2 x (112 KB + ~0.3 KB static + 1 KB reserved)
+//   <= 228 KB.  At the bench shape (LLaMA2-7B, kv length 2049 - 2304: 8 splits of 9 tiles; warp 0 has 3 tiles, warps 1-3
+//   have 2) that is every K tile plus V of tiles 0 - 4 (104 of 144 KB) in flight before the QKV launch resolves; the last
+//   V of each warp is requested as soon as that warp has scored its first tile.
+constexpr int kSlots0 = 5, kSlotsW = 3;
+constexpr int kSlots = kSlots0 + (kAttnWarps - 1) * kSlotsW;
+constexpr int kSmemBytes = kSlots * kHalfBytes;
+// the merge of more than 16 splits stages (m, l) pairs, rescale factors and L of a group in the first 96 KB of the slots
+constexpr int kMergeStageBytes = 96 * 1024;
 constexpr int kChunkAlign = kAttnWarps * kTile;
+static_assert(kSmemBytes <= 112 * 1024 && kMergeStageBytes <= kSmemBytes, "two CTAs per SM");
+
+__device__ __forceinline__ int ring_base(int warp) { return warp == 0 ? 0 : kSlots0 + (warp - 1) * kSlotsW; }
+__device__ __forceinline__ int ring_depth(int warp) { return warp == 0 ? kSlots0 : kSlotsW; }
 
 struct AttnParams {
   const __half* q;
@@ -55,7 +72,7 @@ struct AttnParams {
   unsigned long long* tlc;  // per-CTA stamps (b200_timeline_cta)
   int stream_ef; // K/V bulk copies carry the L2 evict_first policy (B200_KV_EF)
   int even;      // keys dealt out to the splits in whole tiles, evenly (B200_ATTN_EVEN)
-  int pf_early;  // next-stream L2 prefetch as soon as the producer would block instead of after its last tile
+  int pf_early;  // next-stream L2 prefetch as soon as the producer would block instead of after its last copy
 };
 
 // KV-cache layouts are "shared-memory images" so that one 32-position tile is ONE contiguous 8 KB bulk copy:
@@ -63,23 +80,31 @@ struct AttnParams {
 //   V  [B][Hkv][S/32][128][32]   (transposed inside each 32-position block)
 __device__ __forceinline__ int k_swz(int row) { return (row & 1) << 2; }
 
+__device__ __forceinline__ int atomic_add_acq_rel(int* addr, int v) {
+  int old;
+  asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(addr), "r"(v) : "memory");
+  return old;
+}
+
 __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_last;
-  __shared__ __align__(8) uint64_t bars[2 * kStages];
+  __shared__ __align__(8) uint64_t bars[2 * kSlots];
   uint64_t* full = bars;
-  uint64_t* empty = bars + kStages;
-  const int split = blockIdx.x, kvh = blockIdx.y, tok = blockIdx.z;
+  uint64_t* empty = bars + kSlots;
+  // grid (Hkv, n_split, T): CTAs are dispatched kv head fastest, so the last and lightest split (the remainder of the keys)
+  // goes to the SMs the QKV launch frees last
+  const int kvh = blockIdx.x, split = blockIdx.y, tok = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t4 = lane & 3;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
+    for (int s = 0; s < kSlots; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], kAttnWarps);
+      mbar_init(&empty[s], 1);
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  __syncthreads();  // the only CTA-wide barrier
   const int cta_lin = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
   if (threadIdx.x == 0) tl_min(p.tl, 0), tl_cta(p.tlc, cta_lin, 0);
   pdl_launch_dependents();
@@ -106,6 +131,70 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
   }
   const size_t kv_base = ((size_t)brow * p.Hkv + kvh) * p.S * 128;  // same element offset for K and V planes
 
+  if (warp == kAttnWarps) {
+    // ---------------- producer: each warp's halves into that warp's ring ----------------
+    // Lane 0 polls the four rings and issues whatever half is next for a warp whose slot is free, so a full ring never holds
+    // back the halves of the other warps.  Only the tile holding a row the QKV kernel is appending waits for the dependency:
+    // its halves are skipped until nothing else can be issued, then the producer waits once.  The producer takes no part in
+    // the tail and returns when every copy is issued.
+    if (lane == 0) {
+      const bool stream_ef = p.stream_ef != 0;
+      const uint64_t pol = stream_ef ? l2_policy_evict_first() : 0;
+      bool waited = false, pf_done = !(p.next_w && p.next_bytes > 0);
+      auto prefetch_next = [&]() {  // pull the next kernel's weights into L2
+        pf_done = true;
+        const int n_cta = gridDim.x * gridDim.y * gridDim.z;
+        prefetch_next_stream(p.next_w, p.next_bytes, p.next_tiles, p.next_grid, p.next_window, cta_lin, n_cta);
+      };
+      // the QKV kernel appends the rows of every token of this sequence in the launch, not just row pos[tok]: a prompt chunk
+      // whose positions cross a 32-row tile writes into the tile before the one holding pos[tok] as well
+      int first_new = kv_len - 1;
+      for (int j = brow * p.tps; j < min(p.T, (brow + 1) * p.tps); ++j) first_new = min(first_new, p.pos[j]);
+      int next[kAttnWarps], slot[kAttnWarps], n_half[kAttnWarps];  // per ring: next half, its slot, halves in all
+      uint32_t par[kAttnWarps];
+      int left = 0;
+#pragma unroll
+      for (int w = 0; w < kAttnWarps; ++w) {
+        next[w] = 0, slot[w] = ring_base(w), par[w] = 0;
+        n_half[w] = n_tiles > w ? 2 * ((n_tiles - w + kAttnWarps - 1) / kAttnWarps) : 0;
+        left += n_half[w];
+      }
+      while (left > 0) {
+        bool issued = false, held = false;
+#pragma unroll
+        for (int w = 0; w < kAttnWarps; ++w) {
+          if (next[w] == n_half[w]) continue;
+          const int s0 = s_begin + (w + kAttnWarps * (next[w] >> 1)) * kTile;
+          if (!waited && s0 + kTile > first_new) {  // this tile holds a row the QKV kernel is appending right now
+            held = true;
+            continue;
+          }
+          if (!mbar_try_wait(&empty[slot[w]], par[w] ^ 1)) continue;
+          uint8_t* dst = smem + (size_t)slot[w] * kHalfBytes;
+          const __half* src = ((next[w] & 1) ? p.vt : p.kc) + kv_base + (size_t)s0 * 128;
+          mbar_arrive_expect_tx(&full[slot[w]], kHalfBytes);
+          if (stream_ef)
+            bulk_g2s_hint(dst, src, kHalfBytes, &full[slot[w]], pol);
+          else
+            bulk_g2s(dst, src, kHalfBytes, &full[slot[w]]);
+          ++next[w], --left, issued = true;
+          if (++slot[w] == ring_base(w) + ring_depth(w)) slot[w] = ring_base(w), par[w] ^= 1;
+        }
+        if (!issued) {
+          // pf_early: the hint goes out as soon as this producer would block (rings full / dependency), not after its last copy
+          if (p.pf_early && !pf_done) prefetch_next();
+          if (held) {
+            pdl_wait();
+            waited = true;
+          }
+        }
+      }
+      if (!pf_done) prefetch_next();  // own stream issued
+    }
+    return;
+  }
+
+  // ---------------- consumers ----------------
   float oacc[16][4];
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 #pragma unroll
@@ -113,52 +202,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
 #pragma unroll
     for (int i = 0; i < 4; ++i) oacc[j][i] = 0.f;
 
-  if (warp == kAttnWarps) {
-    // ---------------- producer: one (K tile, V tile) pair per stage ----------------
-    // The whole warp walks the loop (only lane 0 issues) and re-converges before the CTA-wide barrier below:
-    // an aligned bar.sync must never be reached by a partial warp.
-    int stage = 0;
-    uint32_t par = 0;
-    bool waited = false, pf_done = !(p.next_w && p.next_bytes > 0);
-    // the QKV kernel appends the rows of every token of this sequence in the launch, not just row pos[tok]: a prompt chunk
-    // whose positions cross a 32-row tile writes into the tile before the one holding pos[tok] as well
-    int first_new = kv_len - 1;
-    for (int j = brow * p.tps; j < min(p.T, (brow + 1) * p.tps); ++j) first_new = min(first_new, p.pos[j]);
-    auto prefetch_next = [&]() {  // pull the next kernel's weights into L2
-      pf_done = true;
-      const int cta = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-      const int n_cta = gridDim.x * gridDim.y * gridDim.z;
-      prefetch_next_stream(p.next_w, p.next_bytes, p.next_tiles, p.next_grid, p.next_window, cta, n_cta);
-    };
-    for (int i = 0; i < n_tiles; ++i) {
-      if (lane == 0) {
-        const int s0 = s_begin + i * kTile;
-        const bool dep = !waited && s0 + kTile > first_new;  // this tile holds a row the QKV kernel is appending right now
-        // pf_early: the hint goes out as soon as this producer would block (ring full / dependency), not after its last tile
-        if (p.pf_early && !pf_done && (i == kStages || dep)) prefetch_next();
-        mbar_wait(&empty[stage], par ^ 1);
-        if (dep) {
-          pdl_wait();
-          waited = true;
-        }
-        uint8_t* dst = smem + (size_t)stage * kStageBytes;
-        mbar_arrive_expect_tx(&full[stage], kStageBytes);
-        if (p.stream_ef) {
-          const uint64_t pol = l2_policy_evict_first();
-          bulk_g2s_hint(dst, p.kc + kv_base + (size_t)s0 * 128, kTile * 256, &full[stage], pol);
-          bulk_g2s_hint(dst + kTile * 256, p.vt + kv_base + (size_t)s0 * 128, kTile * 256, &full[stage], pol);
-        } else {
-          bulk_g2s(dst, p.kc + kv_base + (size_t)s0 * 128, kTile * 256, &full[stage]);
-          bulk_g2s(dst + kTile * 256, p.vt + kv_base + (size_t)s0 * 128, kTile * 256, &full[stage]);
-        }
-      }
-      __syncwarp();
-      if (++stage == kStages) stage = 0, par ^= 1;
-    }
-    if (lane == 0 && !pf_done) prefetch_next();  // own stream issued
-    __syncwarp();
-  } else {
-  // ---------------- consumers ----------------
   pdl_wait();  // q comes from the previous kernel
   if (threadIdx.x == 0) {
     tl_max(p.tl, 1), tl_cta(p.tlc, cta_lin, 1);
@@ -177,23 +220,24 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
       qf[c][hh][0] = v.x, qf[c][hh][1] = v.y, qf[c][hh][2] = v.z, qf[c][hh][3] = v.w;
     }
 
-  // Every consumer warp observes EVERY tile's barrier in order (and releases it), computing only its own tiles
-  // (i % 4 == warp).  A warp that skipped tiles could reach its next use of a stage while that stage's barrier is
-  // still one phase behind; try_wait.parity would then return at once (the same rule that lets a producer through
-  // on its first pass) and the ring would be corrupted -- seen as a rare hang when tiles land out of order.
-  int stage = 0;
+  // This warp's tiles (i % 4 == warp) from its own ring: the K half, then the V half of each.  Every slot of the ring is only
+  // ever waited on by this warp, in the order it was filled, so a wait never meets a barrier one phase behind.
+  int slot = ring_base(warp);
   uint32_t par = 0;
-  for (int i = 0; i < n_tiles; ++i) {
-    mbar_wait(&full[stage], par);
-    if ((i & (kAttnWarps - 1)) != warp) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[stage]);
-      if (++stage == kStages) stage = 0, par ^= 1;
-      continue;
-    }
-    const uint8_t* ks = smem + (size_t)stage * kStageBytes;
-    const uint8_t* vs = ks + kTile * 256;
+  auto release = [&]() {  // hand the slot back to the producer and step to the next one
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[slot]);
+    if (++slot == ring_base(warp) + ring_depth(warp)) slot = ring_base(warp), par ^= 1;
+  };
+  for (int i = warp; i < n_tiles; i += kAttnWarps) {
     const int s0 = s_begin + i * kTile;
+    // K in `slot`, V in the next one (the tile's halves are consecutive in the ring)
+    const bool wrap = slot + 1 == ring_base(warp) + ring_depth(warp);
+    const int vslot = wrap ? ring_base(warp) : slot + 1;
+    mbar_wait(&full[slot], par);
+    mbar_wait(&full[vslot], wrap ? par ^ 1 : par);
+    const uint8_t* ks = smem + (size_t)slot * kHalfBytes;
+    const uint8_t* vs = smem + (size_t)vslot * kHalfBytes;
 
     // ---- S = Q K^T for 4 blocks of 8 positions; block X column n <-> s0 + 8*(n>>1) + 2X + (n&1) ----
     float sacc[4][4];
@@ -209,6 +253,7 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
         mma16816(sacc[X], qf[c][0][2], qf[c][1][2], qf[c][0][3], qf[c][1][3], kb.z, kb.w);
       }
     }
+    release();  // K read: its slot takes this warp's next half while the softmax and P.V run
     // ---- mask + online softmax (rows g and g+8) ----
     float tmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -253,49 +298,47 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
       mma16816(oacc[j], pa[0][0], pa[0][1], pa[0][2], pa[0][3], vb.x, vb.y);
       mma16816(oacc[j], pa[1][0], pa[1][1], pa[1][2], pa[1][3], vb.z, vb.w);
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);
-    if (++stage == kStages) stage = 0, par ^= 1;
+    release();
   }
-  }  // consumers
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     l_run[hh] += __shfl_xor_sync(0xffffffffu, l_run[hh], 1);
     l_run[hh] += __shfl_xor_sync(0xffffffffu, l_run[hh], 2);
   }
-  __syncthreads();  // everyone is done with the rings: reuse them for the in-CTA merge
 
-  float* mo = reinterpret_cast<float*>(smem);                // [4 warps][16 rows][128]
-  float* mml = mo + kAttnWarps * 16 * 128;                   // [4 warps][16 rows][2]
-  if (warp < kAttnWarps) {
+  // ---- in-CTA merge: each warp parks (O, m, l) of the group's rows in its own ring (every copy into it has been consumed),
+  // the four consumer warps meet at one named barrier (the producer is not waited for) and fold the warps in order ----
+  auto part_o = [&](int w) { return reinterpret_cast<float*>(smem + (size_t)ring_base(w) * kHalfBytes); };  // [16][128]
+  auto part_ml = [&](int w) { return part_o(w) + 16 * 128; };                                                // [16][2]
+  {
+    float* mo = part_o(warp);
+    float* mml = part_ml(warp);
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    *reinterpret_cast<float2*>(mo + ((size_t)warp * 16 + g) * 128 + 8 * j + 2 * t4) = make_float2(oacc[j][0], oacc[j][1]);
-    *reinterpret_cast<float2*>(mo + ((size_t)warp * 16 + g + 8) * 128 + 8 * j + 2 * t4) = make_float2(oacc[j][2], oacc[j][3]);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = g + 8 * hh;
+      if (row >= p.n_rep) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<float2*>(mo + (size_t)row * 128 + 8 * j + 2 * t4) = make_float2(oacc[j][2 * hh], oacc[j][2 * hh + 1]);
+      if (t4 == 0) mml[row * 2 + 0] = m_run[hh], mml[row * 2 + 1] = l_run[hh];
+    }
   }
-  if (t4 == 0) {
-    mml[(warp * 16 + g) * 2 + 0] = m_run[0], mml[(warp * 16 + g) * 2 + 1] = l_run[0];
-    mml[(warp * 16 + g + 8) * 2 + 0] = m_run[1], mml[(warp * 16 + g + 8) * 2 + 1] = l_run[1];
-  }
-  }
-  __syncthreads();
+  named_bar_sync(1, kConsumerThreads);
 
-  const int d = threadIdx.x & 127;  // threads 0..127 <-> 128 output dims (the producer warp only tags along)
-  const bool writer = threadIdx.x < 128;
+  const int d = threadIdx.x;  // consumer thread <-> output dim
   for (int h = 0; h < p.n_rep; ++h) {
     float M = -INFINITY;
 #pragma unroll
-    for (int w = 0; w < kAttnWarps; ++w) M = fmaxf(M, mml[(w * 16 + h) * 2]);
+    for (int w = 0; w < kAttnWarps; ++w) M = fmaxf(M, part_ml(w)[h * 2]);
     float L = 0.f, o = 0.f;
 #pragma unroll
     for (int w = 0; w < kAttnWarps; ++w) {
-      const float mw = mml[(w * 16 + h) * 2];
+      const float mw = part_ml(w)[h * 2];
       const float f = (mw == -INFINITY) ? 0.f : exp2f(mw - M);
-      L += mml[(w * 16 + h) * 2 + 1] * f;
-      o += mo[((size_t)w * 16 + h) * 128 + d] * f;
+      L += part_ml(w)[h * 2 + 1] * f;
+      o += part_o(w)[(size_t)h * 128 + d] * f;
     }
     const int hq = kvh * p.n_rep + h;
-    if (!writer) continue;
     if (p.n_split == 1) {
       p.out[((size_t)tok * p.Hq + hq) * 128 + d] = __float2half_rn(o / L);
     } else {
@@ -309,27 +352,24 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     return;
   }
   // ---- cross-split merge by the last CTA to arrive for this (token, kv head) ----
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int old = atomicAdd(&p.counters[tok * p.Hkv + kvh], 1);
-    s_last = (old == p.n_split - 1);
-  }
-  __syncthreads();
+  // One acquire-release add by one thread instead of a sequentially consistent fence in every thread before the count and
+  // again after it: the barrier orders the other consumer threads' partial stores before thread 0's release (release is
+  // cumulative), and the second barrier orders the merging CTA's loads after thread 0's acquire.
+  named_bar_sync(1, kConsumerThreads);  // also: every warp is done reading the parked partials
+  if (threadIdx.x == 0) s_last = atomic_add_acq_rel(&p.counters[tok * p.Hkv + kvh], 1) == p.n_split - 1;
+  named_bar_sync(1, kConsumerThreads);
   if (!s_last) {
     if (threadIdx.x == 0) tl_max(p.tl, 3), tl_cta(p.tlc, cta_lin, 3);
     return;
   }
-  __threadfence();
   // Latency-parallel merge: (1) all (M, L) pairs of the group in one round trip -> smem, (2) one warp per head forms
   // the global max, the rescale factors and L, (3) one warp per head accumulates O with 16 independent 16-byte loads
   // in flight per lane.  (A serial loop over the splits costs one L2 round trip per split: 60 us at 33 splits x 8 heads.)
   if (p.n_split <= 16) {
     // one warp per head, ONE L2 round trip: the (m, l) pairs (lane = split) and all O partials are requested together;
     // same operations in the same order as the general path below (bit-identical results)
-    const int nwarps = blockDim.x >> 5;
     const float2* ml0 = p.ws_ml + ((size_t)tok * p.Hq + (size_t)kvh * p.n_rep) * p.n_split;
-    for (int h = warp; h < p.n_rep; h += nwarps) {
+    for (int h = warp; h < p.n_rep; h += kAttnWarps) {
       const int hq = kvh * p.n_rep + h;
       const float4* base = reinterpret_cast<const float4*>(p.ws_o + ((size_t)tok * p.Hq + hq) * p.n_split * 128) + lane;
       const float2 mlv = lane < p.n_split ? __ldcg(&ml0[h * p.n_split + lane]) : make_float2(-INFINITY, 0.f);
@@ -356,10 +396,9 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
     float* sL = sf + p.n_rep * p.n_split;                              // [n_rep]
     const int nml = p.n_rep * p.n_split;
     const float2* ml0 = p.ws_ml + ((size_t)tok * p.Hq + (size_t)kvh * p.n_rep) * p.n_split;  // heads of a group are adjacent
-    for (int i = threadIdx.x; i < nml; i += blockDim.x) sml[i] = __ldcg(&ml0[i]);
-    __syncthreads();
-    const int nwarps = blockDim.x >> 5;
-    for (int h = warp; h < p.n_rep; h += nwarps) {
+    for (int i = threadIdx.x; i < nml; i += kConsumerThreads) sml[i] = __ldcg(&ml0[i]);
+    named_bar_sync(1, kConsumerThreads);
+    for (int h = warp; h < p.n_rep; h += kAttnWarps) {
       float M = -INFINITY;
       for (int sp = lane; sp < p.n_split; sp += 32) M = fmaxf(M, sml[h * p.n_split + sp].x);
       M = warp_max(M);
@@ -373,8 +412,8 @@ __global__ void __launch_bounds__(kAttnThreads, 2) attn_decode_kernel(const __gr
       L = warp_sum(L);
       if (lane == 0) sL[h] = L;
     }
-    __syncthreads();
-    for (int h = warp; h < p.n_rep; h += nwarps) {
+    named_bar_sync(1, kConsumerThreads);
+    for (int h = warp; h < p.n_rep; h += kAttnWarps) {
       const int hq = kvh * p.n_rep + h;
       const float4* base = reinterpret_cast<const float4*>(p.ws_o + ((size_t)tok * p.Hq + hq) * p.n_split * 128) + lane;
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -406,7 +445,7 @@ using namespace b200;
 
 extern "C" int b200_attn_choose_split(int T, int Hkv, int max_kv_len) {
   if (T <= 0 || Hkv <= 0 || max_kv_len <= 0) return 1;
-  // all CTAs must be co-resident in one wave: 2 CTAs per SM (96 KB ring each)
+  // all CTAs must be co-resident in one wave: 2 CTAs per SM (112 KB of rings each)
   const int target = 2 * sm_count();
   int want = target / (T * Hkv);
   const int max_split = (max_kv_len + kChunkAlign - 1) / kChunkAlign;
@@ -444,8 +483,8 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
   int chunk = (a->max_kv_len + n_split - 1) / n_split;
   chunk = (chunk + kTile - 1) / kTile * kTile;
   n_split = (a->max_kv_len + chunk - 1) / chunk;
-  // the merge of more than 16 splits stages (m, l) pairs, rescale factors and L of a group in the K/V ring
-  if ((size_t)(a->Hq / a->Hkv) * (n_split * 12 + 4) > (size_t)kStages * kStageBytes) {
+  // the merge of more than 16 splits stages (m, l) pairs, rescale factors and L of a group in the slots
+  if ((size_t)(a->Hq / a->Hkv) * (n_split * 12 + 4) > (size_t)kMergeStageBytes) {
     set_error("attn: too many splits for the merge's shared-memory staging");
     return B200_E_INVAL;
   }
@@ -477,7 +516,7 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
   p.tl = timeline_slot();
   p.tlc = timeline_cta_slot();
 
-  const size_t smem = (size_t)kStages * kStageBytes;  // 96 KB ring (also covers the 33 KB merge area)
+  const size_t smem = kSmemBytes;
   static bool configured_dev[16] = {};  // cudaFuncSetAttribute is per device
   int dev = 0;
   cudaGetDevice(&dev);
@@ -491,7 +530,7 @@ extern "C" int b200_attn_decode(const b200_attn_args_t* a, b200_stream_t stream)
     configured = true;
   }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(n_split, a->Hkv, a->T);
+  cfg.gridDim = dim3(a->Hkv, n_split, a->T);
   cfg.blockDim = dim3(kAttnThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = static_cast<cudaStream_t>(stream);
